@@ -293,7 +293,13 @@ __global__ void __launch_bounds__(WPB * 32) cost_batch_warp_kernel(
   }
   const double dt = opt_time ? xb[nvar - 1] : t.knot_span;
   double fo, gr[3], gdt;
-  eval_warp<FAST>(g, dist, p, t, tc + b, n, mask, q, dt, lane, fo, gr, gdt);
+  if constexpr (FAST) {
+    TrajFast tf;
+    load_traj_fast(tc + b, tf);
+    eval_warp_fast(g, dist, p, tf, tc + b, n, mask, q, dt, lane, fo, gr, gdt);
+  } else {
+    eval_warp(g, dist, p, t, tc + b, n, mask, q, dt, lane, fo, gr, gdt);
+  }
   double* gb = grad + (int64_t)b * nvar;
   if (lane < n) {
     gb[3 * lane] = gr[0];

@@ -38,7 +38,7 @@ __device__ __forceinline__ double dot3(const V3& a, const V3& b) {
 // history element (slot, component k) of this lane: [slot][k][lane], conflict-free
 #define HIDX(slot, k) ((slot) * 96 + (k) * 32 + lane)
 
-__global__ void __launch_bounds__(WPB * 32) optimize_warp_kernel(
+__global__ void __launch_bounds__(WPB * 32, 3) optimize_warp_kernel(
     Geom g, const float* __restrict__ dist, FuelOptParams p, const FuelTrajConst* __restrict__ tc, int n,
     int mask, int B, FuelSolveParams sp, double* __restrict__ x, double* __restrict__ fbest,
     int* __restrict__ neval_out) {
@@ -53,8 +53,9 @@ __global__ void __launch_bounds__(WPB * 32) optimize_warp_kernel(
   double* S = hist + (size_t)w * 2 * m * 96;
   double* Y = S + (size_t)m * 96;
   double* xb = x + (int64_t)b * nvar;
-  TrajRegs t;
-  load_traj(tc + b, t);
+  TrajFast t;  // the faithful evaluator's constants are loaded after the loop, for the final evaluation only
+  load_traj_fast(tc + b, t);
+  const double knot_span = tc[b].knot_span;
 
   // variables of this lane: control point (lane < n), dt in component 0 of lane n
   const bool is_pt = lane < n;
@@ -81,9 +82,9 @@ __global__ void __launch_bounds__(WPB * 32) optimize_warp_kernel(
   }
 
   auto evaluate = [&](const V3& xx, double& fo, V3& go) {
-    const double dtv = opt_time ? __shfl_sync(0xffffffffu, xx.v[0], n) : t.knot_span;
+    const double dtv = opt_time ? __shfl_sync(0xffffffffu, xx.v[0], n) : knot_span;
     double gr[3], gdt;
-    eval_warp<true>(g, dist, p, t, tc + b, n, mask, xx.v, dtv, lane, fo, gr, gdt);
+    eval_warp_fast(g, dist, p, t, tc + b, n, mask, xx.v, dtv, lane, fo, gr, gdt);
     go.v[0] = is_pt ? gr[0] : (is_dt ? gdt : 0.0);
     go.v[1] = is_pt ? gr[1] : 0.0;
     go.v[2] = is_pt ? gr[2] : 0.0;
@@ -259,9 +260,11 @@ __global__ void __launch_bounds__(WPB * 32) optimize_warp_kernel(
 #pragma unroll
     for (int k = 0; k < 3; ++k) XB.v[k] = is_pt ? xb[3 * lane + k] : 0.0;
     if (is_dt) XB.v[0] = xb[nvar - 1];
-    const double dtv = opt_time ? __shfl_sync(0xffffffffu, XB.v[0], n) : t.knot_span;
+    TrajRegs tr;
+    load_traj(tc + b, tr);
+    const double dtv = opt_time ? __shfl_sync(0xffffffffu, XB.v[0], n) : tr.knot_span;
     double fo, gr[3], gdt;
-    eval_warp<false>(g, dist, p, t, tc + b, n, mask, XB.v, dtv, lane, fo, gr, gdt);
+    eval_warp(g, dist, p, tr, tc + b, n, mask, XB.v, dtv, lane, fo, gr, gdt);
     if (lane == 0) fbest[b] = fo;
   }
   if (lane == 0) neval_out[b] = neval;
@@ -297,65 +300,121 @@ __device__ __forceinline__ float transpose_reduce32(float (&v)[32], int lane) {
   return v[0];
 }
 
-// floats of shared memory per warp (a multiple of 4: the history is float4)
-#define GRAM_FLOATS(M) ((2 * (M) * 32 * 4 + 2 * (M) * (M) + 3 * (M) + 32 + 3) / 4 * 4)
+// Shared memory per warp, in floats: the S and Y history (M*32 float4 each, ring order); the Gram data in AGE order (row j
+// belongs to the j-th newest pair, rows padded to GROW floats so that a row is two float4 reads): SY[M][GROW], YY[M][GROW],
+// U[GROW], W[GROW], RHO[GROW]; the 32 sums of the last batched reduction; then the box bounds as doubles (lb 3*32 | ub 3*32),
+// and in FUEL_PROF builds four cycle counters.
+constexpr int GROW = 8;
+#define GRAM_FLOATS(M) (2 * (M) * 32 * 4 + 2 * (M) * GROW + 3 * GROW + 32)
+#ifdef FUEL_PROF
+#define PROF_FLOATS 8
+#else
+#define PROF_FLOATS 0
+#endif
+#define SOLVER_FLOATS(M) (GRAM_FLOATS(M) + 2 * 3 * 32 * 2 + PROF_FLOATS)
+constexpr int SOLVER_WPB = 4;         // warps (trajectories) per CTA of optimize_gram_kernel
+constexpr int SOLVER_SM_WARPS = 12;   // resident warps per SM its registers are sized for: 65536 / (12 * 32) = 170 each
+
+#ifdef FUEL_PROF
+// FUEL_PROF builds: clock64() cycles of optimize_gram_kernel per phase, summed over all warps of the launches since the
+// last read (fuelgpu_debug_solver_prof): [0] evaluation, [1] Armijo steps (trial point, acceptance test), [2] s/y,
+// projection of the new gradient, batched reduction and Gram update, [3] two-loop recursion + direction, [4] whole kernel,
+// [5] evaluations, [6] L-BFGS iterations, [7] warps.  The per-warp sums live in shared memory (lane 0 adds), so the
+// stamps hold no registers across the loop beyond the start time of the open phase.
+__device__ unsigned long long g_solver_prof[8];
+#define PROF_T(v) const long long v = clock64()
+#define PROF_ADD(i, v) \
+  do { if (lane == 0) PROF[i] += clock64() - (v); } while (0)
+#else
+#define PROF_T(v) do {} while (0)
+#define PROF_ADD(i, v) do {} while (0)
+#endif
+
+// row j of an age-ordered Gram matrix (GROW floats, 16-byte aligned) as two float4 reads
+template <int M>
+__device__ __forceinline__ void gram_row(const float* __restrict__ r, float (&o)[M]) {
+  const float4 a = *reinterpret_cast<const float4*>(r), c = *reinterpret_cast<const float4*>(r + 4);
+  const float t[8] = { a.x, a.y, a.z, a.w, c.x, c.y, c.z, c.w };
+#pragma unroll
+  for (int i = 0; i < M; ++i) o[i] = t[i];
+}
 
 template <int M>  // history length, compile time: every recursion loop has static bounds (5*M + 1 <= 32 values per batch)
-__global__ void __launch_bounds__(WPB * 32) optimize_gram_kernel(
+__global__ void __launch_bounds__(SOLVER_WPB * 32, SOLVER_SM_WARPS / SOLVER_WPB) optimize_gram_kernel(
     Geom g, const float* __restrict__ dist, FuelOptParams p, const FuelTrajConst* __restrict__ tc, int n,
     int mask, int B, FuelSolveParams sp, double* __restrict__ x, double* __restrict__ fbest,
     int* __restrict__ neval_out) {
   static_assert(5 * M + 1 <= 32, "the batched reduction holds 32 values");
+  static_assert(M <= GROW && 2 * (M - 1) * (M - 1) + (M - 1) <= 64, "Gram rows hold GROW values; the age shift moves <= 2 per lane");
   constexpr int MAXM = M;  // (shadows the file-level bound: Gram arrays are M wide here)
-  extern __shared__ double hist[];  // per warp, as floats: S M*32 float4 | Y M*32 float4 | SY M*M | YY M*M | rho,u,w M | red 32
+  extern __shared__ double hist[];  // per warp: SOLVER_FLOATS(M) floats, layout above
   const int lane = threadIdx.x & 31;
   const int w = threadIdx.x >> 5;
-  const int b = blockIdx.x * WPB + w;
+  const int b = blockIdx.x * SOLVER_WPB + w;
   if (b >= B) return;
+#ifdef FUEL_PROF
+  int n_iter = 0;
+  PROF_T(t_kernel);
+#endif
   const bool opt_time = (mask & FUELGPU_MINTIME) != 0;
   const int nvar = opt_time ? 3 * n + 1 : 3 * n;
   constexpr int m = M;
-  float4* S4 = reinterpret_cast<float4*>(hist) + (size_t)w * (GRAM_FLOATS(M) / 4);
+  float4* S4 = reinterpret_cast<float4*>(hist) + (size_t)w * (SOLVER_FLOATS(M) / 4);
   float4* Y4 = S4 + M * 32;
-  float* SYg = reinterpret_cast<float*>(Y4 + M * 32);
-  float* YYg = SYg + MAXM * MAXM;
-  float* RHO = YYg + MAXM * MAXM;
-  float* Ug = RHO + MAXM;
-  float* Wg = Ug + MAXM;
-  float* RED = Wg + MAXM;  // the 32 sums of the last batched reduction
+  float* SYa = reinterpret_cast<float*>(Y4 + M * 32);  // SYa[j * GROW + i] = s_j . y_i, j and i ages (0 = newest)
+  float* YYa = SYa + M * GROW;                           // YYa[j * GROW + i] = y_j . y_i
+  float* Ua = YYa + M * GROW;                            // s_j . pg, y_j . pg for the current projected gradient
+  float* Wa = Ua + GROW;
+  float* Ra = Wa + GROW;                                 // 1 / s_j . y_j
+  float* RED = Ra + GROW;  // the 32 sums of the last batched reduction
+  // the box bounds of this lane's variables, [k][lane]: read once per projection and Armijo step, so they need no registers
+  // across the evaluation
+  double* LB = reinterpret_cast<double*>(RED + 32);
+  double* UB = LB + 3 * 32;
+#ifdef FUEL_PROF
+  unsigned long long* PROF = reinterpret_cast<unsigned long long*>(UB + 3 * 32);
+  if (lane < 4) PROF[lane] = 0;
+#endif
+  // ages >= cnt are masked in the recursion; zeros keep them finite
+  for (int i = lane; i < 2 * M * GROW + 3 * GROW; i += 32) SYa[i] = 0.f;
   double* xb = x + (int64_t)b * nvar;
-  TrajRegs t;
-  load_traj(tc + b, t);
+  TrajFast t;  // the faithful evaluator's constants are loaded after the loop, for the final evaluation only
+  load_traj_fast(tc + b, t);
+  const double knot_span = tc[b].knot_span;
 
   const bool is_pt = lane < n;
   const bool is_dt = opt_time && lane == n;
-  V3 X, lb, ub;
+  V3 X;
 #pragma unroll
   for (int k = 0; k < 3; ++k) {
     X.v[k] = 0.0;
-    lb.v[k] = 0.0;
-    ub.v[k] = 0.0;
+    double lo = 0.0, hi = 0.0;
     if (is_pt) {
       const double bmin = g.box_mind[k] + 0.1, bmax = g.box_maxd[k] - 0.1;
       double c = xb[3 * lane + k];
       c = fmax(fmin(c, bmax), bmin);  // :199-203
       X.v[k] = c;
-      lb.v[k] = fmax(c - 10.0, bmin);  // :208-214
-      ub.v[k] = fmin(c + 10.0, bmax);
+      lo = fmax(c - 10.0, bmin);  // :208-214
+      hi = fmin(c + 10.0, bmax);
     }
+    if (is_dt && k == 0) {
+      X.v[0] = xb[nvar - 1];
+      lo = 0.0;  // :215-218
+      hi = 5.0;
+    }
+    LB[k * 32 + lane] = lo;
+    UB[k * 32 + lane] = hi;
   }
-  if (is_dt) {
-    X.v[0] = xb[nvar - 1];
-    lb.v[0] = 0.0;  // :215-218
-    ub.v[0] = 5.0;
-  }
+  __syncwarp();
   auto evaluate = [&](const V3& xx, double& fo, V3& go) {
-    const double dtv = opt_time ? __shfl_sync(0xffffffffu, xx.v[0], n) : t.knot_span;
+    PROF_T(t_eval);
+    const double dtv = opt_time ? __shfl_sync(0xffffffffu, xx.v[0], n) : knot_span;
     double gr[3], gdt;
-    eval_warp<true>(g, dist, p, t, tc + b, n, mask, xx.v, dtv, lane, fo, gr, gdt);
+    eval_warp_fast(g, dist, p, t, tc + b, n, mask, xx.v, dtv, lane, fo, gr, gdt);
     go.v[0] = is_pt ? gr[0] : (is_dt ? gdt : 0.0);
     go.v[1] = is_pt ? gr[1] : 0.0;
     go.v[2] = is_pt ? gr[2] : 0.0;
+    PROF_ADD(0, t_eval);
   };
   auto store_best = [&](const V3& xx, double fv) {
     if (is_pt) {
@@ -369,7 +428,7 @@ __global__ void __launch_bounds__(WPB * 32) optimize_gram_kernel(
   auto project = [&](const V3& xx, const V3& gg, V3& pg, bool actv[3]) {
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
-      actv[k] = (xx.v[k] <= lb.v[k] && gg.v[k] > 0.0) || (xx.v[k] >= ub.v[k] && gg.v[k] < 0.0);
+      actv[k] = (xx.v[k] <= LB[k * 32 + lane] && gg.v[k] > 0.0) || (xx.v[k] >= UB[k * 32 + lane] && gg.v[k] < 0.0);
       pg.v[k] = actv[k] ? 0.0 : gg.v[k];
     }
   };
@@ -401,45 +460,47 @@ __global__ void __launch_bounds__(WPB * 32) optimize_gram_kernel(
       }
       break;
     }
-    // ---- two-loop recursion on fp32 scalars (every lane the same values; Gram data by broadcast reads).  The Gram
-    // entries come out of an fp32 reduction, so fp32 arithmetic on them loses nothing; the result is only the search
-    // direction -- acceptance (F, Armijo) and the iterate stay fp64.
-    float a[M], cs[M], cy[M];
-    int slot[M];
+#ifdef FUEL_PROF
+    ++n_iter;
+#endif
+    PROF_T(t_rec);
+    // ---- two-loop recursion on fp32 scalars (every lane the same values).  The Gram entries come out of an fp32
+    // reduction, so fp32 arithmetic on them loses nothing; the result is only the search direction -- acceptance (F,
+    // Armijo) and the iterate stay fp64.  The Gram data is stored by age, so every index below is static: the rows are
+    // vector reads issued together before the recursion, ages >= cnt are masked by rho = 0, and each sum is written so
+    // that the value computed last enters last (one FMA and one multiply per slot on the dependent chain).
+    float a[M], cs[M], cy[M], rho[M], u[M], wv[M], gsy[M][M], gyy[M][M];
+    int slot[M];  // ring slot of the j-th newest pair (the S/Y vectors stay in ring order)
+    gram_row<M>(Ua, u);
+    gram_row<M>(Wa, wv);
+    gram_row<M>(Ra, rho);
 #pragma unroll
     for (int j = 0; j < M; ++j) {
+      gram_row<M>(SYa + j * GROW, gsy[j]);
+      gram_row<M>(YYa + j * GROW, gyy[j]);
       int sl = head - 1 - j;
       if (sl < 0) sl += m;
       slot[j] = j < cnt ? sl : 0;
-      a[j] = 0.f;
-      cs[j] = 0.f;
-      cy[j] = 0.f;
+      if (j >= cnt) rho[j] = 0.f;
     }
 #pragma unroll
     for (int j = 0; j < M; ++j) {  // newest -> oldest
-      if (j < cnt) {
-        float acc = Ug[slot[j]];
+      float acc = u[j];
 #pragma unroll
-        for (int i = 0; i < M; ++i)
-          if (i < j) acc -= a[i] * SYg[slot[j] * M + slot[i]];
-        a[j] = RHO[slot[j]] * acc;
-      }
+      for (int i = 0; i < j; ++i) acc -= a[i] * gsy[j][i];
+      a[j] = j < cnt ? rho[j] * acc : 0.f;
     }
     float gd = gamma * pgn2;  // accumulates pg.r
 #pragma unroll
     for (int j = M - 1; j >= 0; --j) {  // oldest -> newest
-      if (j < cnt) {
-        float yq = Wg[slot[j]];
+      float yq = wv[j];
 #pragma unroll
-        for (int i = 0; i < M; ++i)
-          if (i < cnt) yq -= a[i] * YYg[slot[j] * M + slot[i]];
-        float acc = gamma * yq;
+      for (int i = 0; i < M; ++i) yq -= a[i] * gyy[j][i];  // a is complete: off the chain
+      float acc = gamma * yq;
 #pragma unroll
-        for (int i = 0; i < M; ++i)
-          if (i > j && i < cnt) acc += cs[i] * SYg[slot[i] * M + slot[j]];
-        cs[j] = a[j] - RHO[slot[j]] * acc;
-        cy[j] = -gamma * a[j];
-      }
+      for (int i = M - 1; i > j; --i) acc += cs[i] * gsy[i][j];
+      cs[j] = j < cnt ? a[j] - rho[j] * acc : 0.f;
+      cy[j] = -gamma * a[j];
     }
     // direction: r = gamma pg + sum_j cs_j s_j + cy_j y_j ;  d = -r off the active bounds ;  g.d = -pg.r
     float R[3];
@@ -447,8 +508,8 @@ __global__ void __launch_bounds__(WPB * 32) optimize_gram_kernel(
     for (int k = 0; k < 3; ++k) R[k] = gamma * pgf[k];
 #pragma unroll
     for (int j = 0; j < M; ++j) {
+      gd += cs[j] * u[j] + cy[j] * wv[j];
       if (j < cnt) {
-        gd += cs[j] * Ug[slot[j]] + cy[j] * Wg[slot[j]];
         const float4 st = S4[slot[j] * 32 + lane], yt = Y4[slot[j] * 32 + lane];
         R[0] += cs[j] * st.x + cy[j] * yt.x;
         R[1] += cs[j] * st.y + cy[j] * yt.y;
@@ -466,20 +527,24 @@ __global__ void __launch_bounds__(WPB * 32) optimize_gram_kernel(
       cnt = 0;
     }
     double step = cnt == 0 ? (double)fminf(1.f, rsqrtf(pgn2)) : 1.0;
+    PROF_ADD(3, t_rec);
 
     // ---- Armijo backtracking on the projected path ----
     bool accepted = false;
     V3 XN, GN;
     double FN = 0.0;
     while (neval < sp.max_eval) {
+      PROF_T(t_trial);
       bool clipped = false;
 #pragma unroll
       for (int k = 0; k < 3; ++k) {
-        const double xt = X.v[k] + step * D.v[k];
-        clipped = clipped || xt > ub.v[k] || xt < lb.v[k];
-        XN.v[k] = fmax(fmin(xt, ub.v[k]), lb.v[k]);
+        const double xt = X.v[k] + step * D.v[k], lo = LB[k * 32 + lane], hi = UB[k * 32 + lane];
+        clipped = clipped || xt > hi || xt < lo;
+        XN.v[k] = fmax(fmin(xt, hi), lo);
       }
+      PROF_ADD(1, t_trial);
       evaluate(XN, FN, GN);
+      PROF_T(t_test);
       ++neval;
       if (FN < best) {  // costFunction :698-704
         best = FN;
@@ -492,18 +557,17 @@ __global__ void __launch_bounds__(WPB * 32) optimize_gram_kernel(
         for (int k = 0; k < 3; ++k) dx.v[k] = XN.v[k] - X.v[k];
         dec = wsum_x(d3(G, dx));
       }
-      if (FN <= F + 1e-4 * dec) {
-        accepted = true;
-        break;
-      }
-      step *= 0.5;
-      if (step < 1e-12) break;
+      accepted = FN <= F + 1e-4 * dec;
+      if (!accepted) step *= 0.5;
+      PROF_ADD(1, t_test);
+      if (accepted || step < 1e-12) break;
     }
     if (!accepted) {
       if (!exact) break;
       cnt = 0;
       continue;
     }
+    PROF_T(t_red);
     float sf[3], yf[3];
     bool small = true;
 #pragma unroll
@@ -548,38 +612,61 @@ __global__ void __launch_bounds__(WPB * 32) optimize_gram_kernel(
       }
     }
     const float mine = transpose_reduce32(v, lane);  // lane l: the sum of value l
+    // a kept pair makes every stored pair one age older: the entries of ages 0..M-2 (SY and YY blocks, RHO) move to
+    // ages 1..M-1, at most two per lane, read here before anything is written
+    constexpr int NB = (M - 1) * (M - 1), NMOVE = 2 * NB + (M - 1);
+    float mv[2];
+    int mv_dst[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int e = lane + 32 * r;
+      int src = -1, dst = -1;
+      if (e < 2 * NB) {
+        const int blk = e < NB ? 0 : 1, o = e - blk * NB, row = o / (M - 1), col = o - row * (M - 1);
+        src = blk * M * GROW + row * GROW + col;  // SYa / YYa relative to SYa
+        dst = src + GROW + 1;
+      } else if (e < NMOVE) {
+        src = (Ra - SYa) + (e - 2 * NB);
+        dst = src + 1;
+      }
+      mv[r] = src >= 0 ? SYa[src] : 0.f;
+      mv_dst[r] = dst;
+    }
     RED[lane] = mine;
     __syncwarp();
     const float sy = RED[0], yy = RED[1], ss = RED[2];
     pgn2 = RED[3];
     const bool keep = sy > 1e-10f * sqrtf(ss) * sqrtf(yy);
-    // Gram update, one lane per value: value 6 + 5j + q belongs to the j-th newest pair
+    // Gram update, one lane per value: value 6 + 5j + q belongs to the j-th newest pair, which becomes age j+1 if the new
+    // pair is kept (the new pair is age 0: row and column 0)
     if (lane >= 6) {
       const int j = (lane - 6) / 5, q = (lane - 6) - 5 * j;
-      if (j < cnt) {
-        int st = head - 1 - j;
-        if (st < 0) st += m;
-        if (st != drop) {
-          if (q == 3) Ug[st] = mine;
-          if (q == 4) Wg[st] = mine;
-          if (keep) {
-            if (q == 0) SYg[head * M + st] = mine;  // s_new . y_t
-            if (q == 1) SYg[st * M + head] = mine;  // s_t . y_new
-            if (q == 2) {
-              YYg[head * M + st] = mine;
-              YYg[st * M + head] = mine;
-            }
+      if (j < cnt && j < M - 1) {  // (age M-1 was left out of the reduction: it is dropped either way)
+        const int age = keep ? j + 1 : j;
+        if (q == 3) Ua[age] = mine;
+        if (q == 4) Wa[age] = mine;
+        if (keep) {
+          if (q == 0) SYa[age] = mine;         // s_new . y_t
+          if (q == 1) SYa[age * GROW] = mine;  // s_t . y_new
+          if (q == 2) {
+            YYa[age] = mine;
+            YYa[age * GROW] = mine;
           }
         }
       }
     } else if (keep) {
       if (lane == 0) {
-        SYg[head * M + head] = sy;
-        RHO[head] = __fdividef(1.f, sy);
+        SYa[0] = sy;
+        Ra[0] = __fdividef(1.f, sy);
       }
-      if (lane == 1) YYg[head * M + head] = yy;
-      if (lane == 4) Ug[head] = mine;
-      if (lane == 5) Wg[head] = mine;
+      if (lane == 1) YYa[0] = yy;
+      if (lane == 4) Ua[0] = mine;
+      if (lane == 5) Wa[0] = mine;
+    }
+    if (keep) {  // rows/columns 1..M-1 of SY and YY, RHO 1..M-1: disjoint from the entries written above
+#pragma unroll
+      for (int r = 0; r < 2; ++r)
+        if (mv_dst[r] >= 0) SYa[mv_dst[r]] = mv[r];
     }
     if (keep) {
       S4[head * 32 + lane] = make_float4(sf[0], sf[1], sf[2], 0.f);
@@ -587,8 +674,13 @@ __global__ void __launch_bounds__(WPB * 32) optimize_gram_kernel(
       gamma = __fdividef(sy, yy);
       head = head + 1 == m ? 0 : head + 1;
       if (cnt < m) ++cnt;
+    } else if (drop >= 0) {
+      // the oldest pair was left out of this reduction, so its s.pg and y.pg still belong to the previous projected
+      // gradient: it leaves the history (its slot is the next one written)
+      cnt = m - 1;
     }
     __syncwarp();
+    PROF_ADD(2, t_red);
     if (!exact && __all_sync(0xffffffffu, small)) break;  // xtol_rel, :173
   }
   {
@@ -597,12 +689,24 @@ __global__ void __launch_bounds__(WPB * 32) optimize_gram_kernel(
 #pragma unroll
     for (int k = 0; k < 3; ++k) XB.v[k] = is_pt ? xb[3 * lane + k] : 0.0;
     if (is_dt) XB.v[0] = xb[nvar - 1];
-    const double dtv = opt_time ? __shfl_sync(0xffffffffu, XB.v[0], n) : t.knot_span;
+    TrajRegs tr;
+    load_traj(tc + b, tr);
+    const double dtv = opt_time ? __shfl_sync(0xffffffffu, XB.v[0], n) : tr.knot_span;
     double fo, gr[3], gdt;
-    eval_warp<false>(g, dist, p, t, tc + b, n, mask, XB.v, dtv, lane, fo, gr, gdt);
+    eval_warp(g, dist, p, tr, tc + b, n, mask, XB.v, dtv, lane, fo, gr, gdt);
     if (lane == 0) fbest[b] = fo;
   }
   if (lane == 0) neval_out[b] = neval;
+#ifdef FUEL_PROF
+  if (lane == 0) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) atomicAdd(&g_solver_prof[i], PROF[i]);
+    atomicAdd(&g_solver_prof[4], (unsigned long long)(clock64() - t_kernel));
+    atomicAdd(&g_solver_prof[5], (unsigned long long)neval);
+    atomicAdd(&g_solver_prof[6], (unsigned long long)n_iter);
+    atomicAdd(&g_solver_prof[7], 1ull);
+  }
+#endif
 }
 
 }  // namespace
@@ -626,12 +730,23 @@ int bspline_optimize_batch_dev_impl(FuelMap* m, int B, int n_pts, int mask, cons
                                                                         x_dev, fbest_dev, neval_dev);
   } else {
     constexpr int GM = 6;
-    const size_t smem = (size_t)WPB * GRAM_FLOATS(GM) * sizeof(float);
+    const size_t smem = (size_t)SOLVER_WPB * SOLVER_FLOATS(GM) * sizeof(float);
     FUEL_CUDA(m, cudaFuncSetAttribute(optimize_gram_kernel<GM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    optimize_gram_kernel<GM><<<(B + WPB - 1) / WPB, WPB * 32, smem, m->stream>>>(m->g, m->dist, *p, tc_dev, n_pts, mask, B, *sp,
+    optimize_gram_kernel<GM><<<(B + SOLVER_WPB - 1) / SOLVER_WPB, SOLVER_WPB * 32, smem, m->stream>>>(m->g, m->dist, *p, tc_dev, n_pts, mask, B, *sp,
                                                                             x_dev, fbest_dev, neval_dev);
   }
   FUEL_LAUNCHES(m, 1);
   FUEL_CUDA(m, cudaGetLastError());
   return 0;
 }
+
+#ifdef FUEL_PROF
+// debug-only (FUEL_PROF builds): the per-phase cycle sums of optimize_gram_kernel (layout at g_solver_prof); reading
+// them resets them
+extern "C" __attribute__((visibility("default"))) int fuelgpu_debug_solver_prof(unsigned long long* out, int n) {
+  if (n > 8) n = 8;
+  if (cudaMemcpyFromSymbol(out, g_solver_prof, sizeof(unsigned long long) * n) != cudaSuccess) return -1;
+  const unsigned long long zero[8] = {};
+  return cudaMemcpyToSymbol(g_solver_prof, zero, sizeof(zero)) == cudaSuccess ? 0 : -1;
+}
+#endif
