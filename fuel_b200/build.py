@@ -7,8 +7,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libfuelgpu.so")
-SOURCES = ["api.cu", "esdf.cu", "esdf_tile.cu", "sharded.cu", "frontier.cu", "bspline.cu", "bspline_solve.cu", "fusion.cu", "viewpoints.cu"]
-FMAD_OK = {"bspline_solve.cu", "esdf.cu", "esdf_tile.cu", "sharded.cu"}  # files whose arithmetic need not follow the host rounding sequence
+SOURCES = ["api.cu", "esdf.cu", "esdf_tile.cu", "sharded.cu", "frontier.cu", "bspline.cu", "bspline_solve.cu", "bspline_solve_long.cu",
+           "fusion.cu", "viewpoints.cu"]
+FMAD_OK = {"bspline_solve.cu", "bspline_solve_long.cu", "esdf.cu", "esdf_tile.cu", "sharded.cu"}  # files whose arithmetic need not follow the host rounding sequence
 HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "bspline_eval.cuh"),
            os.path.join(ROOT, "include", "fuelgpu.h")]
 

@@ -239,7 +239,7 @@ int fuelgpu_map_destroy(FuelMap* m) {
   for (int i = 0; i < 2; ++i)
     if (m->esdf_ev[i]) cudaEventDestroy(m->esdf_ev[i]);
   void* ptrs[] = { m->occ,       m->dist,      m->dist_neg, m->flag,   m->esdf_rec,
-                   m->esdf_p[0], m->esdf_p[1], m->stage,    m->bs_buf, m->fr_scr };
+                   m->esdf_p[0], m->esdf_p[1], m->stage,    m->bs_buf, m->fr_scr, m->bs_grad };
   for (void* p : ptrs)
     if (p) cudaFree(p);
   for (int t = 0; t < T_COUNT; ++t) {

@@ -312,6 +312,43 @@ __global__ void __launch_bounds__(WPB * 32) cost_batch_warp_kernel(
   }
 }
 
+// FUELGPU_COST_FAST_EVAL for 32 < n <= 64: the two-points-per-lane evaluator of the long-trajectory solver
+__global__ void __launch_bounds__(WPB * 32) cost_batch_warp2_kernel(
+    Geom g, const float* __restrict__ dist, FuelOptParams p, const FuelTrajConst* __restrict__ tc, int n,
+    int mask, int B, const double* __restrict__ x, double* __restrict__ f, double* __restrict__ grad) {
+  const int lane = threadIdx.x & 31;
+  const int b = blockIdx.x * WPB + (threadIdx.x >> 5);
+  if (b >= B) return;
+  const bool opt_time = (mask & FUELGPU_MINTIME) != 0;
+  const int nvar = opt_time ? 3 * n + 1 : 3 * n;
+  const double* xb = x + (int64_t)b * nvar;
+  double q[2][3];
+#pragma unroll
+  for (int s = 0; s < 2; ++s) {
+    const int i = 32 * s + lane;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) q[s][k] = i < n ? xb[3 * i + k] : 0.0;
+  }
+  const double dt = opt_time ? xb[nvar - 1] : tc[b].knot_span;
+  TrajFast tf;
+  load_traj_fast(tc + b, tf);
+  double fo, gr[2][3], gdt;
+  eval_warp_fast2(g, dist, p, tf, tc + b, n, mask, q, dt, lane, fo, gr, gdt);
+  double* gb = grad + (int64_t)b * nvar;
+#pragma unroll
+  for (int s = 0; s < 2; ++s) {
+    const int i = 32 * s + lane;
+    if (i < n) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) gb[3 * i + k] = gr[s][k];
+    }
+  }
+  if (lane == 0) {
+    f[b] = fo;
+    if (opt_time) gb[nvar - 1] = gdt;
+  }
+}
+
 }  // namespace
 
 int bspline_cost_batch_dev_impl(FuelMap* m, int B, int n_pts, int mask, const FuelOptParams* p,
@@ -320,9 +357,10 @@ int bspline_cost_batch_dev_impl(FuelMap* m, int B, int n_pts, int mask, const Fu
   if (B <= 0) return 0;
   const bool fast = (mask & FUELGPU_COST_FAST_EVAL) != 0;
   mask &= ~FUELGPU_COST_FAST_EVAL;
-  if (fast && n_pts > 32)
-    return fuel_fail(m, FUELGPU_EUNSUPPORTED, "FUELGPU_COST_FAST_EVAL needs n_pts <= 32 (the solver's evaluator)");
-  if (fast) {
+  if (fast && n_pts > 32) {
+    cost_batch_warp2_kernel<<<(B + WPB - 1) / WPB, WPB * 32, 0, m->stream>>>(m->g, m->dist, *p, tc_dev, n_pts, mask, B,
+                                                                            x_dev, f_dev, grad_dev);
+  } else if (fast) {
     cost_batch_warp_kernel<true><<<(B + WPB - 1) / WPB, WPB * 32, 0, m->stream>>>(m->g, m->dist, *p, tc_dev, n_pts,
                                                                               mask, B, x_dev, f_dev, grad_dev);
   } else if (n_pts <= 32) {

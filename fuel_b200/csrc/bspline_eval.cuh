@@ -619,4 +619,221 @@ __device__ __forceinline__ void eval_warp_fast(const Geom& g, const float* __res
   f_out = f;
 }
 
+// =========================================================================================
+// Two points per lane (32 < n <= 64): control point i lives on lane i % 32, in slot i / 32 (strided), so
+// q[s][k] of lane l is coordinate k of point 32 s + l.  Points n..63 are inactive (finite, gradient zero).
+// dt is a warp-uniform scalar on every lane.  The same terms, arithmetic and outputs as eval_warp_fast: each
+// point's terms run in its own slot, the contributions to points i+1..i+3 go up the warp in one vector per
+// offset and slot, and all cost and dt-gradient partials meet in one merged butterfly.
+// =========================================================================================
+
+// point i + d (slot s of this lane, 1 <= d <= 3): the next slot's lane (lane + d - 32) for the last d lanes of
+// slot 0.  Lane L sends slot 0 to lane L - d, or slot 1 to lane L - d + 32: one shuffle per slot.  (Slot 1 of
+// the last d lanes, points >= 64, reads a finite value of no point; every term that uses it is masked.)
+__device__ __forceinline__ double fwd2(const double (&q)[2][3], int s, int k, int d, int lane) {
+  const double src = (s == 0 && lane >= d) ? q[0][k] : q[1][k];
+  return __shfl_sync(0xffffffffu, src, (lane + d) & 31);
+}
+// what point i - d added to point i (o[s][k]: what this lane's point of slot s adds to its point + d): for slot 0
+// none below lane d, for slot 1 the last d lanes of slot 0
+__device__ __forceinline__ double back2(const double (&o)[2][3], int s, int k, int d, int lane) {
+  const double src = (s == 1 && lane < 32 - d) ? o[1][k] : o[0][k];
+  const double r = __shfl_sync(0xffffffffu, src, (lane - d) & 31);
+  return (s == 0 && lane < d) ? 0.0 : r;
+}
+// coordinate k of point j (warp-uniform j < 64) in every lane
+__device__ __forceinline__ double point2(const double (&q)[2][3], int j, int k) {
+  return __shfl_sync(0xffffffffu, (j >> 5) ? q[1][k] : q[0][k], j & 31);
+}
+
+__device__ __forceinline__ void eval_warp_fast2(const Geom& g, const float* __restrict__ dist, const FuelOptParams& p,
+                                                const TrajFast& t, const FuelTrajConst* __restrict__ tc, int n,
+                                                int mask, const double (&q)[2][3], double dt, int lane, double& f_out,
+                                                double (&gr)[2][3], double& gdt) {
+  const bool opt_time = (mask & FUELGPU_MINTIME) != 0;
+  double f_lane = 0.0, gdt_lane = 0.0;  // per-lane partial sums, reduced once at the end
+  const double dt_inv = 1.0 / dt;
+  const double dt_inv2 = dt_inv * dt_inv, inv2dt = 0.5 * dt_inv;
+  // this lane's own gradient rows, and what its terms add to the rows of points i+1, i+2, i+3
+  double own[2][3], o1[2][3], o2[2][3], o3[2][3];
+#pragma unroll
+  for (int s = 0; s < 2; ++s) {
+    const int i = 32 * s + lane;
+    double q1[3], q2[3], q3[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      q1[k] = fwd2(q, s, k, 1, lane);
+      q2[k] = fwd2(q, s, k, 2, lane);
+      q3[k] = fwd2(q, s, k, 3, lane);
+      own[s][k] = o1[s][k] = o2[s][k] = o3[s][k] = 0.0;
+    }
+    const double* qi = q[s];
+    if ((mask & FUELGPU_SMOOTHNESS) && i <= n - 4) {  // calcSmoothnessCost :255-282
+      double ji[3];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) ji[k] = (q3[k] - 3 * q2[k] + 3 * q1[k] - qi[k]) * t.inv_pt;
+      f_lane += p.ld_smooth * (ji[0] * ji[0] + ji[1] * ji[1] + ji[2] * ji[2]);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const double tj = p.ld_smooth * 2 * ji[k] * t.inv_pt;
+        own[s][k] -= tj;
+        o1[s][k] += 3.0 * tj;
+        o2[s][k] -= 3.0 * tj;
+        o3[s][k] += tj;
+      }
+    }
+    if ((mask & FUELGPU_DISTANCE) && i < n) {  // calcDistanceCost :284-306
+      double dg[3];
+      const double d = dev_dist_with_grad_fast(g, dist, qi, dg);
+      const double n2 = dg[0] * dg[0] + dg[1] * dg[1] + dg[2] * dg[2];
+      if (n2 > 1e-8) {
+        const double rn = rsqrt(n2);
+        dg[0] *= rn;
+        dg[1] *= rn;
+        dg[2] *= rn;
+      }
+      if (d < p.dist0) {
+        f_lane += p.ld_dist * ((d - p.dist0) * (d - p.dist0));
+#pragma unroll
+        for (int k = 0; k < 3; ++k) own[s][k] += p.ld_dist * (2.0 * (d - p.dist0) * dg[k]);
+      }
+    }
+    if (mask & FUELGPU_FEASIBILITY) {  // calcFeasibilityCost :308-353
+      double c = 0.0, gtl = 0.0;
+      const bool vv = i <= n - 2, va = i <= n - 3;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const double vi = (q1[k] - qi[k]) * dt_inv;
+        const double vd = fabs(vi) - p.max_vel;
+        if (vv && vd > 0.0) {
+          c += vd * vd;
+          const double tv = 2 * vd * (vi > 0 ? 1.0 : -1.0) * dt_inv;
+          if (opt_time) gtl += tv * (-vi);
+          own[s][k] -= p.ld_feasi * tv;
+          o1[s][k] += p.ld_feasi * tv;
+        }
+      }
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const double ai = (q2[k] - 2 * q1[k] + qi[k]) * dt_inv2;
+        const double ad = fabs(ai) - p.max_acc;
+        if (va && ad > 0.0) {
+          c += ad * ad;
+          const double ta = 2 * ad * (ai > 0 ? 1.0 : -1.0) * dt_inv2;
+          if (opt_time) gtl += ta * ai * (-2) * dt;
+          own[s][k] += p.ld_feasi * ta;
+          o1[s][k] -= 2.0 * p.ld_feasi * ta;
+          o2[s][k] += p.ld_feasi * ta;
+        }
+      }
+      f_lane += p.ld_feasi * c;
+      gdt_lane += p.ld_feasi * gtl;
+    }
+    // calcStartCost :355-391 on point 0 and calcEndCost :393-431 on point n-3, from the points they hold
+    const bool do_start = (mask & FUELGPU_START) && i == 0, do_end = (mask & FUELGPU_END) && i == n - 3;
+    if (do_start || do_end) {
+      const double(*st)[3] = do_start ? tc->start : tc->end;
+      const double w_pos = do_start ? 10.0 : 1.0, ld = do_start ? p.ld_start : p.ld_end;
+      const bool use_v = do_start || t.n_end >= 2, use_a = do_start || t.n_end == 3;
+      double cost = 0.0, gt = 0.0;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        const double dv = q2[k] - qi[k], da = qi[k] - 2 * q1[k] + q2[k];
+        const double dqp = 1 / 6.0 * (qi[k] + 4 * q1[k] + q2[k]) - __ldg(&st[0][k]);
+        const double dqv = use_v ? inv2dt * dv - __ldg(&st[1][k]) : 0.0;
+        const double dqa = use_a ? dt_inv2 * da - __ldg(&st[2][k]) : 0.0;
+        cost += w_pos * dqp * dqp + dqv * dqv + dqa * dqa;
+        gt -= dqv * dv * dt_inv2 + dqa * da * dt_inv2 * dt_inv;
+        const double ep = ld * 2.0 * w_pos * dqp, ev = ld * 2.0 * dqv, ea = ld * 2.0 * dqa;
+        own[s][k] += ep * (1 / 6.0) - ev * inv2dt + ea * dt_inv2;
+        o1[s][k] += ep * (4 / 6.0) - 2.0 * ea * dt_inv2;
+        o2[s][k] += ep * (1 / 6.0) + ev * inv2dt + ea * dt_inv2;
+      }
+      f_lane += ld * cost;
+      if (opt_time) gdt_lane += ld * gt;
+    }
+  }
+#pragma unroll
+  for (int s = 0; s < 2; ++s)
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+      gr[s][k] = own[s][k] + back2(o1, s, k, 1, lane) + back2(o2, s, k, 2, lane) + back2(o3, s, k, 3, lane);
+
+  if (mask & FUELGPU_GUIDE) {  // calcGuideCost :462-475
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+      const int i = 32 * s + lane;
+      if (i >= p.order && i < n - p.order) {
+        double d[3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) d[k] = q[s][k] - tc->guide[i - p.order][k];
+        f_lane += p.ld_guide * (d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) gr[s][k] += p.ld_guide * (2 * d[k]);
+      }
+    }
+  }
+  double f = 0.0;  // warp-uniform terms
+  gdt = 0.0;
+  if (mask & FUELGPU_WAYPOINTS) {  // calcWaypointsCost :433-457
+    double cost = 0.0;
+    for (int w = 0; w < t.n_waypt; ++w) {
+      const int idx = tc->waypt_idx[w];
+      double dq[3];
+#pragma unroll
+      for (int k = 0; k < 3; ++k)
+        dq[k] = 1 / 6.0 * (point2(q, idx, k) + 4 * point2(q, idx + 1, k) + point2(q, idx + 2, k)) - tc->waypt[w][k];
+      cost += dq[0] * dq[0] + dq[1] * dq[1] + dq[2] * dq[2];
+#pragma unroll
+      for (int s = 0; s < 2; ++s) {
+        const int r = 32 * s + lane - idx;  // this point's place in the waypoint's stencil
+        if (r >= 0 && r <= 2) {
+          const double c = r == 1 ? 8.0 / 6.0 : 2.0 / 6.0;
+#pragma unroll
+          for (int k = 0; k < 3; ++k) gr[s][k] += p.ld_waypt * (dq[k] * c);
+        }
+      }
+    }
+    f += p.ld_waypt * cost;
+  }
+  if (mask & FUELGPU_VIEWCONS) {  // calcViewCost :477-502: one control point, every lane evaluates it (no reduction)
+    const int idx = tc->view_idx;
+    if (idx >= 0 && idx < n) {
+      double qi[3], gv[3];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) qi[k] = point2(q, idx, k);
+      const double c = view_cost_point(qi, tc->view_pt, tc->view_dir, p.wnl, gv);
+      f += p.ld_view * c;
+      if (lane == (idx & 31)) {
+        const int s = idx >> 5;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) gr[s][k] += p.ld_view * gv[k];
+      }
+    }
+  }
+  if (mask & FUELGPU_MINTIME) {  // calcTimeCost :504-516
+    const double duration = (n - p.order) * dt;
+    double cost = duration;
+    double gt = (double)(n - p.order);
+    if (t.time_lb > 0 && duration < t.time_lb) {
+      const double w_lb = 10;
+      cost += w_lb * (duration - t.time_lb) * (duration - t.time_lb);
+      gt += w_lb * 2 * (duration - t.time_lb) * (n - p.order);
+    }
+    f += p.ld_time * cost;
+    gdt += p.ld_time * gt;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    f_lane += __shfl_down_sync(0xffffffffu, f_lane, o);
+    gdt_lane += __shfl_down_sync(0xffffffffu, gdt_lane, o);
+  }
+  f += __shfl_sync(0xffffffffu, f_lane, 0);
+  if (opt_time) gdt += __shfl_sync(0xffffffffu, gdt_lane, 0);
+#pragma unroll
+  for (int s = 0; s < 2; ++s)
+    if (32 * s + lane >= n) gr[s][0] = gr[s][1] = gr[s][2] = 0.0;
+  f_out = f;
+}
+
 }  // namespace

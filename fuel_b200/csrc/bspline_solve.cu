@@ -716,8 +716,8 @@ int bspline_optimize_batch_dev_impl(FuelMap* m, int B, int n_pts, int mask, cons
                                     double* x_dev, double* fbest_dev, int32_t* neval_dev) {
   if (B <= 0) return 0;
   const int need = n_pts + ((mask & FUELGPU_MINTIME) ? 1 : 0);
-  if (need > 32)
-    return fuel_fail(m, FUELGPU_EUNSUPPORTED, "optimize_batch supports at most 32 lanes (n_pts + dt)");
+  if (need > 32)  // two control points per lane (bspline_solve_long.cu)
+    return bspline_optimize_long_impl(m, B, n_pts, mask, p, tc_dev, sp, x_dev, fbest_dev, neval_dev);
   static int use_vec = -1;  // FUELGPU_SOLVER=vec selects the vector-space two-loop recursion (A/B, debugging)
   if (use_vec < 0) {
     const char* e = getenv("FUELGPU_SOLVER");

@@ -63,6 +63,8 @@ struct FuelMap {
   size_t bs_bytes;
   void* bs_pin;  // page-locked bounce buffer for the host-facing B-spline calls
   size_t bs_pin_bytes;
+  void* bs_grad;  // gradient output of the faithful re-evaluation after the long-trajectory solver (discarded)
+  size_t bs_grad_bytes;
   void* fr_scr;  // device scratch of the small frontier-side calls (is_changed, viewpoints), grown on demand
   size_t fr_scr_bytes;
   int bs_pend_B, bs_pend_nvar;  // optimize_batch_begin issued, _end outstanding (B == 0: none)
@@ -164,6 +166,9 @@ int bspline_cost_batch_dev_impl(FuelMap* m, int B, int n_pts, int mask, const Fu
 int bspline_optimize_batch_dev_impl(FuelMap* m, int B, int n_pts, int mask, const FuelOptParams* p,
                                     const FuelTrajConst* tc_dev, const FuelSolveParams* sp,
                                     double* x_dev, double* fbest_dev, int32_t* neval_dev);
+int bspline_optimize_long_impl(FuelMap* m, int B, int n_pts, int mask, const FuelOptParams* p,
+                               const FuelTrajConst* tc_dev, const FuelSolveParams* sp, double* x_dev,
+                               double* fbest_dev, int32_t* neval_dev);
 
 // getDistWithGrad on the device (sdf_map.cpp:497-536); shared by esdf.cu and bspline.cu
 __device__ __forceinline__ double dev_get_distance(const Geom& g, const float* __restrict__ dist,

@@ -306,7 +306,7 @@ FUELGPU_API int fuelgpu_frontier_changed_counts(FuelMap* map, int32_t n_clusters
 #define FUELGPU_MINTIME (1 << 8)
 /* not a cost term: evaluate with the solver loop's evaluator (fuelgpu_bspline_optimize_batch runs it: fp32
  * trilinear lerps on the fp32 ESDF samples, reciprocals, FMA contraction) instead of the faithful one; same
- * 1e-4 parity bar, n_pts <= 32 */
+ * 1e-4 parity bar, n_pts <= 64 (above 32 points: the two-points-per-lane evaluator of the long-trajectory solver) */
 #define FUELGPU_COST_FAST_EVAL (1 << 30)
 
 /* BsplineOptimizer::setParam (bspline_optimizer.cpp:25-57) */
@@ -354,7 +354,9 @@ FUELGPU_API int fuelgpu_bspline_cost_batch_dev(FuelMap* map, int32_t B, int32_t 
  * whole batch on the device.  NLopt (third party, LD_LBFGS) is replaced by a projected
  * L-BFGS run per trajectory inside one persistent kernel; iterate-level parity with NLopt
  * is unpinned (SURVEY 8c), the CPU twin is oracle/orc_optimize_batch.
- * x [B][nvar] in/out (best_variable_), f_best [B], n_eval [B]. */
+ * x [B][nvar] in/out (best_variable_), f_best [B], n_eval [B].  n_pts <= 64: up to 32 lanes (n_pts + dt) one
+ * control point per lane, above that two per lane (and f_best is then exactly what fuelgpu_bspline_cost_batch returns
+ * for the returned x). */
 typedef struct {
   int32_t max_eval; /* max_iteration_num_[id]  (algorithm.xml:184-187) */
   int32_t lbfgs_m;  /* history pairs, <= 8                              */
