@@ -9,6 +9,8 @@ importing works anywhere, but every operation needs libfuelgpu.so and an sm_90 d
 from ._lib import FuelGpuError, lib  # noqa: F401
 from .bspline_optimizer import BsplineOptimizer  # noqa: F401
 from .frontier_finder import Frontier, FrontierFinder  # noqa: F401
+from .non_uniform_bspline import NonUniformBspline  # noqa: F401
 from .sdf_map import EDTEnvironment, SDFMap  # noqa: F401
 
-__all__ = ["SDFMap", "EDTEnvironment", "FrontierFinder", "Frontier", "BsplineOptimizer", "FuelGpuError", "lib"]
+__all__ = ["SDFMap", "EDTEnvironment", "FrontierFinder", "Frontier", "BsplineOptimizer", "NonUniformBspline",
+           "FuelGpuError", "lib"]

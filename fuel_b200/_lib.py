@@ -72,6 +72,18 @@ class FuelSolveParams(C.Structure):
 SOLVE_EXACT_EVALS = 1
 
 
+class FuelTrajCheckParams(C.Structure):
+    _fields_ = [("max_vel", C.c_double), ("max_acc", C.c_double), ("t_now", C.c_double)]
+
+
+class FuelTrajReport(C.Structure):
+    _fields_ = [("duration", C.c_double), ("jerk", C.c_double), ("ratio", C.c_double), ("distance", C.c_double),
+                ("safe", C.c_int32), ("feasible", C.c_int32), ("n_checked", C.c_int32), ("reserved", C.c_int32)]
+
+
+CHECK_MAX_SAMPLES = 1 << 20
+
+
 # every symbol include/fuelgpu.h declares: name -> (restype, argtypes)
 _vp, _i32, _i64, _dbl = C.c_void_p, C.c_int32, C.c_int64, C.c_double
 SIGNATURES = {
@@ -145,6 +157,10 @@ SIGNATURES = {
     "fuelgpu_sharded_esdf_allgather": (C.c_int, [_vp, _vp, _vp, _vp]),
     "fuelgpu_sharded_esdf_destroy": (C.c_int, [_vp]),
     "fuelgpu_esdf_set_from_slabs_dev": (C.c_int, [_vp, _vp, _i32]),
+    "fuelgpu_bspline_check_batch": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, C.POINTER(FuelTrajCheckParams), _vp, _vp]),
+    "fuelgpu_bspline_check_batch_dev": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, C.POINTER(FuelTrajCheckParams), _vp,
+                                                  _vp]),
+    "fuelgpu_bspline_evaluate_batch": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _i32, _vp, _i32, _vp]),
 }
 
 _lib = None

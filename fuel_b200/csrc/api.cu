@@ -239,7 +239,7 @@ int fuelgpu_map_destroy(FuelMap* m) {
   for (int i = 0; i < 2; ++i)
     if (m->esdf_ev[i]) cudaEventDestroy(m->esdf_ev[i]);
   void* ptrs[] = { m->occ,       m->dist,      m->dist_neg, m->flag,   m->esdf_rec,
-                   m->esdf_p[0], m->esdf_p[1], m->stage,    m->bs_buf, m->fr_scr, m->bs_grad };
+                   m->esdf_p[0], m->esdf_p[1], m->stage,    m->bs_buf, m->fr_scr, m->bs_grad, m->tc_buf };
   for (void* p : ptrs)
     if (p) cudaFree(p);
   for (int t = 0; t < T_COUNT; ++t) {
@@ -951,6 +951,104 @@ int fuelgpu_bspline_optimize_batch(FuelMap* m, int32_t B, int32_t n_pts, int32_t
   int rc = fuelgpu_bspline_optimize_batch_begin(m, B, n_pts, mask, p, traj, solve, x);
   if (rc) return rc;
   return fuelgpu_bspline_optimize_batch_end(m, x, f_best, n_eval);
+}
+
+static int check_traj_args(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar, bool has_x, bool has_dt) {
+  if (!m) return fuel_fail(nullptr, FUELGPU_EINVAL, "null map");
+  if (B < 0) return fuel_fail(m, FUELGPU_EINVAL, "negative batch");
+  if (n_pts < 4 || n_pts > FUELGPU_MAX_PTS) return fuel_fail(m, FUELGPU_EINVAL, "n_pts must be in 4..64");
+  if (nvar == 3 * n_pts + 1) {
+    if (has_dt) return fuel_fail(m, FUELGPU_EINVAL, "nvar == 3*n_pts + 1 carries dt in x: pass dt = NULL");
+  } else if (nvar == 3 * n_pts) {
+    if (B > 0 && !has_dt) return fuel_fail(m, FUELGPU_EINVAL, "nvar == 3*n_pts needs dt[B]");
+  } else {
+    return fuel_fail(m, FUELGPU_EINVAL, "nvar must be 3*n_pts or 3*n_pts + 1");
+  }
+  if (B > 0 && !has_x) return fuel_fail(m, FUELGPU_EINVAL, "null argument");
+  return 0;
+}
+
+static int ensure_tc(FuelMap* m, size_t bytes) {
+  if (bytes <= m->tc_bytes) return 0;
+  if (m->tc_buf) cudaFree(m->tc_buf);
+  m->tc_buf = nullptr;
+  m->tc_bytes = 0;
+  FUEL_CUDA(m, cudaMalloc(&m->tc_buf, bytes));
+  m->tc_bytes = bytes;
+  return 0;
+}
+
+static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+int fuelgpu_bspline_check_batch_dev(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar, const void* x_dev,
+                                    const void* dt_dev, const FuelTrajCheckParams* p, void* report_dev, void* best_dev) {
+  int rc = check_traj_args(m, B, n_pts, nvar, x_dev != nullptr, dt_dev != nullptr);
+  if (rc) return rc;
+  if (!p || !best_dev || (B > 0 && !report_dev)) return fuel_fail(m, FUELGPU_EINVAL, "null argument");
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  tbegin(m, T_CHECK);
+  rc = traj_check_impl(m, B, n_pts, nvar, (const double*)x_dev, (const double*)dt_dev, p, (FuelTrajReport*)report_dev,
+                       (int32_t*)best_dev);
+  tend(m, T_CHECK);
+  return rc;
+}
+
+int fuelgpu_bspline_check_batch(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar, const double* x, const double* dt,
+                                const FuelTrajCheckParams* p, FuelTrajReport* report, int32_t best[2]) {
+  int rc = check_traj_args(m, B, n_pts, nvar, x != nullptr, dt != nullptr);
+  if (rc) return rc;
+  if (!p || !best || (B > 0 && !report)) return fuel_fail(m, FUELGPU_EINVAL, "null argument");
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  const size_t xb = align256(sizeof(double) * (size_t)B * nvar), db = align256(sizeof(double) * (size_t)B);
+  const size_t rb = align256(sizeof(FuelTrajReport) * (size_t)B);
+  rc = ensure_tc(m, xb + db + rb + 256);
+  if (rc) return rc;
+  uint8_t* base = (uint8_t*)m->tc_buf;
+  double* d_x = (double*)base;
+  double* d_dt = dt ? (double*)(base + xb) : nullptr;
+  FuelTrajReport* d_rep = (FuelTrajReport*)(base + xb + db);
+  int32_t* d_best = (int32_t*)(base + xb + db + rb);
+  if (B > 0) {
+    FUEL_CUDA(m, cudaMemcpyAsync(d_x, x, sizeof(double) * (size_t)B * nvar, cudaMemcpyHostToDevice, m->stream));
+    if (dt) FUEL_CUDA(m, cudaMemcpyAsync(d_dt, dt, sizeof(double) * (size_t)B, cudaMemcpyHostToDevice, m->stream));
+  }
+  tbegin(m, T_CHECK);
+  rc = traj_check_impl(m, B, n_pts, nvar, d_x, d_dt, p, d_rep, d_best);
+  tend(m, T_CHECK);
+  if (rc) return rc;
+  if (B > 0)
+    FUEL_CUDA(m, cudaMemcpyAsync(report, d_rep, sizeof(FuelTrajReport) * (size_t)B, cudaMemcpyDeviceToHost, m->stream));
+  FUEL_CUDA(m, cudaMemcpyAsync(best, d_best, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, m->stream));
+  FUEL_CUDA(m, cudaStreamSynchronize(m->stream));
+  return 0;
+}
+
+int fuelgpu_bspline_evaluate_batch(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar, const double* x, const double* dt,
+                                   int32_t n_t, const double* t, int32_t deriv, double* out) {
+  int rc = check_traj_args(m, B, n_pts, nvar, x != nullptr, dt != nullptr);
+  if (rc) return rc;
+  if (n_t < 0 || deriv < 0 || deriv > 2) return fuel_fail(m, FUELGPU_EINVAL, "n_t must be >= 0 and deriv 0, 1 or 2");
+  if (B == 0 || n_t == 0) return 0;
+  if (!t || !out) return fuel_fail(m, FUELGPU_EINVAL, "null argument");
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  const size_t nt = (size_t)B * n_t;
+  const size_t xb = align256(sizeof(double) * (size_t)B * nvar), db = align256(sizeof(double) * (size_t)B);
+  const size_t tb = align256(sizeof(double) * nt);
+  rc = ensure_tc(m, xb + db + tb + sizeof(double) * 3 * nt);
+  if (rc) return rc;
+  uint8_t* base = (uint8_t*)m->tc_buf;
+  double* d_x = (double*)base;
+  double* d_dt = dt ? (double*)(base + xb) : nullptr;
+  double* d_t = (double*)(base + xb + db);
+  double* d_out = (double*)(base + xb + db + tb);
+  FUEL_CUDA(m, cudaMemcpyAsync(d_x, x, sizeof(double) * (size_t)B * nvar, cudaMemcpyHostToDevice, m->stream));
+  if (dt) FUEL_CUDA(m, cudaMemcpyAsync(d_dt, dt, sizeof(double) * (size_t)B, cudaMemcpyHostToDevice, m->stream));
+  FUEL_CUDA(m, cudaMemcpyAsync(d_t, t, sizeof(double) * nt, cudaMemcpyHostToDevice, m->stream));
+  rc = traj_evaluate_impl(m, B, n_pts, nvar, d_x, d_dt, n_t, d_t, deriv, d_out);
+  if (rc) return rc;
+  FUEL_CUDA(m, cudaMemcpyAsync(out, d_out, sizeof(double) * 3 * nt, cudaMemcpyDeviceToHost, m->stream));
+  FUEL_CUDA(m, cudaStreamSynchronize(m->stream));
+  return 0;
 }
 
 

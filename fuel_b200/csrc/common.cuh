@@ -23,7 +23,7 @@ struct Geom {
   double box_mind[3], box_maxd[3];
 };
 
-enum { T_ESDF = 0, T_FRONTIER = 1, T_BSPLINE = 2, T_UPLOAD = 3, T_DOWNLOAD = 4, T_COUNT = 8 };
+enum { T_ESDF = 0, T_FRONTIER = 1, T_BSPLINE = 2, T_UPLOAD = 3, T_DOWNLOAD = 4, T_CHECK = 5, T_COUNT = 8 };
 
 struct FrontierState;  // frontier.cu
 struct FusionState;    // fusion.cu
@@ -71,6 +71,8 @@ struct FuelMap {
   size_t bs_pend_off;           // offset of the result block inside bs_pin
   long long launches;  // kernels launched so far
   char err[512];
+  void* tc_buf;  // device scratch of the host-facing trajectory check / evaluate calls, grown on demand
+  size_t tc_bytes;
 };
 
 extern thread_local char g_fuelgpu_err[512];
@@ -169,6 +171,11 @@ int bspline_optimize_batch_dev_impl(FuelMap* m, int B, int n_pts, int mask, cons
 int bspline_optimize_long_impl(FuelMap* m, int B, int n_pts, int mask, const FuelOptParams* p,
                                const FuelTrajConst* tc_dev, const FuelSolveParams* sp, double* x_dev,
                                double* fbest_dev, int32_t* neval_dev);
+// traj_check.cu: NonUniformBspline checks / checkTrajCollision / selectBestTraj, and evaluateDeBoorT
+int traj_check_impl(FuelMap* m, int B, int n_pts, int nvar, const double* x_dev, const double* dt_dev,
+                    const FuelTrajCheckParams* p, FuelTrajReport* rep_dev, int32_t* best_dev);
+int traj_evaluate_impl(FuelMap* m, int B, int n_pts, int nvar, const double* x_dev, const double* dt_dev, int n_t,
+                       const double* t_dev, int deriv, double* out_dev);
 
 // getDistWithGrad on the device (sdf_map.cpp:497-536); shared by esdf.cu and bspline.cu
 __device__ __forceinline__ double dev_get_distance(const Geom& g, const float* __restrict__ dist,

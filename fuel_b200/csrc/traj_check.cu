@@ -1,0 +1,310 @@
+// traj_check.cu -- verdicts on a batch of uniform cubic B-splines, on the map's main stream behind the solver:
+// NonUniformBspline::evaluateDeBoorT / getDerivative / getTimeSum / getJerk / checkFeasibility / checkRatio
+// (bspline/src/non_uniform_bspline.cpp), FastPlannerManager::checkTrajCollision (planner_manager.cpp:96-118) and
+// selectBestTraj (:476-482).
+//
+// Built with -fmad=false: every output equals the reference's fp64 arithmetic bit for bit.
+//  - knots are the running sum of setUniformBspline (:16-32), u[i] = u[i-1] + dt, not i*dt;
+//  - derivative control points are (p * (P[i+1] - P[i])) / (u[i+p+1] - u[i+1]) per element (:77-86), the derivative
+//    spline keeps the parent's knots minus the first and last (:97-106);
+//  - getJerk sums (dt_i * c) * c sequentially, i outer, axis inner (:283-298);
+//  - the collision scan's fut_t is the running sum 0.02, 0.04, ... of the reference's loop; a warp evaluates 32
+//    samples at a time and a ballot finds the first one at which the sequential loop stops.
+// One warp per trajectory; its control points, knots and derivative control points sit in shared memory.
+#include "common.cuh"
+
+namespace {
+
+constexpr int TC_WPB = 4;                       // warps per CTA
+constexpr int TC_KNOTS = FUELGPU_MAX_PTS + 4;   // knots of a cubic with n_pts control points
+constexpr unsigned FULL = 0xffffffffu;
+
+struct SplineSmem {
+  double P[FUELGPU_MAX_PTS][3];  // control points
+  double Q[FUELGPU_MAX_PTS][3];  // getDerivative() control points (n - 1)
+  double R[FUELGPU_MAX_PTS][3];  // getDerivative().getDerivative() control points (n - 2)
+  double U[TC_KNOTS];            // knots u_[0..n+3]
+  double J[FUELGPU_MAX_PTS][3];  // getJerk's terms (n - 3 rows)
+};
+
+// The spline of warp `b`: control points from x [B][nvar] (dt in x[b][3n] when nvar == 3n + 1, else dt[b]), the
+// knot vector, and the control points of the first and second derivative.
+__device__ void load_spline(SplineSmem& s, int b, int n, int nvar, const double* __restrict__ x,
+                            const double* __restrict__ dtv, int lane) {
+  const double* xb = x + (size_t)b * nvar;
+  for (int e = lane; e < 3 * n; e += 32) s.P[e / 3][e % 3] = xb[e];
+  if (lane == 0) {
+    const double dt = nvar == 3 * n + 1 ? xb[3 * n] : dtv[b];
+    const int m = n + 3;  // m_ = n_ + p_ + 1 with n_ = n - 1
+    for (int i = 0; i <= m; ++i) s.U[i] = i <= 3 ? (double)(-3 + i) * dt : s.U[i - 1] + dt;
+  }
+  __syncwarp();
+  for (int e = lane; e < 3 * (n - 1); e += 32) {
+    const int i = e / 3, j = e % 3;
+    s.Q[i][j] = (3.0 * (s.P[i + 1][j] - s.P[i][j])) / (s.U[i + 4] - s.U[i + 1]);
+  }
+  __syncwarp();
+  for (int e = lane; e < 3 * (n - 2); e += 32) {  // derivative knots u'[k] = u[k + 1], p' = 2
+    const int i = e / 3, j = e % 3;
+    s.R[i][j] = (2.0 * (s.Q[i + 1][j] - s.Q[i][j])) / (s.U[i + 4] - s.U[i + 2]);
+  }
+  __syncwarp();
+}
+
+// evaluateDeBoor (:51-71) of a degree-p spline with nc control points C and knots Uk (m = nc + p), at u; the knot
+// search starts at *k (>= p), which is exact whenever every knot below it is < the clamped u, and returns its stop.
+template <int p>
+__device__ __forceinline__ void deboor(const double (*C)[3], const double* Uk, int nc, double u, int* kio,
+                                       double out[3]) {
+  const int m = nc + p;
+  const double lo = Uk[p], hi = Uk[m - p];
+  double ub = lo < u ? u : lo;  // std::max(u_(p_), u)
+  ub = hi < ub ? hi : ub;       // std::min(.., u_(m_ - p_))
+  int k = *kio;
+  while (k < m - p - 1 && Uk[k + 1] < ub) ++k;
+  *kio = k;
+  double d[p + 1][3];
+#pragma unroll
+  for (int i = 0; i <= p; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) d[i][j] = C[k - p + i][j];
+#pragma unroll
+  for (int r = 1; r <= p; ++r)
+#pragma unroll
+    for (int i = p; i >= r; --i) {
+      const double alpha = (ub - Uk[i + k - p]) / (Uk[i + 1 + k - r] - Uk[i + k - p]);
+#pragma unroll
+      for (int j = 0; j < 3; ++j) d[i][j] = (1 - alpha) * d[i - 1][j] + alpha * d[i][j];
+    }
+#pragma unroll
+  for (int j = 0; j < 3; ++j) out[j] = d[p][j];
+}
+
+// SDFMap::getInflateOccupancy(pos) == 1 (sdf_map.h:217-226): posToIndex then isInMap(idx); outside the map is -1,
+// not a hit.  Comparing the floored doubles with [0, n-1] is the int conversion plus the bounds test of the
+// reference for every value (an out-of-range or NaN conversion lands outside the map on x86-64 as well).
+__device__ __forceinline__ bool inflate_hit(const Geom& g, const uint8_t* __restrict__ occ, const double pt[3]) {
+  const double fx = floor((pt[0] - g.origin[0]) * g.res_inv);
+  const double fy = floor((pt[1] - g.origin[1]) * g.res_inv);
+  const double fz = floor((pt[2] - g.origin[2]) * g.res_inv);
+  if (!(fx >= 0.0 && fy >= 0.0 && fz >= 0.0 && fx <= g.nx - 1 && fy <= g.ny - 1 && fz <= g.nz - 1)) return false;
+  return (__ldg(occ + addr_of(g, (int)fx, (int)fy, (int)fz)) & 4) != 0;
+}
+
+__device__ __forceinline__ double warp_max_ref(double v) {  // std::max reduction of non-NaN partials
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    const double w = __shfl_xor_sync(FULL, v, o);
+    v = v < w ? w : v;
+  }
+  return v;
+}
+
+__global__ void __launch_bounds__(TC_WPB * 32) traj_check_kernel(Geom g, const uint8_t* __restrict__ occ, int B, int n,
+                                                                 int nvar, const double* __restrict__ x,
+                                                                 const double* __restrict__ dtv, FuelTrajCheckParams prm,
+                                                                 FuelTrajReport* __restrict__ rep) {
+  __shared__ SplineSmem sm[TC_WPB];
+  const int lane = threadIdx.x & 31;
+  const int b = blockIdx.x * TC_WPB + (threadIdx.x >> 5);
+  if (b >= B) return;
+  SplineSmem& s = sm[threadIdx.x >> 5];
+  load_spline(s, b, n, nvar, x, dtv, lane);
+
+  // checkRatio / checkFeasibility (:135-160, :443-487): the velocity rows are the derivative control points
+  const double lim_v = prm.max_vel + 1e-4, lim_a = prm.max_acc + 1e-4;
+  double mv = -1.0, ma = -1.0;
+  bool fea = true;
+  for (int e = lane; e < 3 * (n - 1); e += 32) {
+    const double v = fabs(s.Q[e / 3][e % 3]);
+    fea = fea && !(v > lim_v);
+    mv = mv < v ? v : mv;
+  }
+  for (int e = lane; e < 3 * (n - 2); e += 32) {
+    const int i = e / 3, j = e % 3;
+    const double a = (6.0 * ((s.P[i + 2][j] - s.P[i + 1][j]) / (s.U[i + 5] - s.U[i + 2]) -
+                             (s.P[i + 1][j] - s.P[i][j]) / (s.U[i + 4] - s.U[i + 1]))) /
+                     (s.U[i + 4] - s.U[i + 2]);
+    const double v = fabs(a);
+    fea = fea && !(v > lim_a);
+    ma = ma < v ? v : ma;
+  }
+  // getJerk's terms: third-derivative control points (knots u''[k] = u[k + 2], p'' = 1) times their knot interval
+  for (int e = lane; e < 3 * (n - 3); e += 32) {
+    const int i = e / 3, j = e % 3;
+    const double w = s.U[i + 4] - s.U[i + 3];
+    const double c = (1.0 * (s.R[i + 1][j] - s.R[i][j])) / w;
+    s.J[i][j] = w * c * c;
+  }
+  mv = warp_max_ref(mv);
+  ma = warp_max_ref(ma);
+  fea = __all_sync(FULL, fea);
+  __syncwarp();
+
+  // checkTrajCollision's loop (planner_manager.cpp:96-118), 32 samples per step
+  const double duration = s.U[n] - s.U[3];
+  const double t_now = prm.t_now;
+  double cur[3];
+  int k0 = 3;
+  deboor<3>(s.P, s.U, n, t_now + s.U[3], &k0, cur);
+  int kstart = 3;
+  double ft_base = 0.0, r_carry = 0.0;  // fut_t of the sample before this step (0 + 0.02 = 0.02 exactly), its radius
+  int n_checked = 0, safe = 1;
+  double distance = -1.0;
+  for (int base = 0;; base += 32) {
+    double ft = ft_base, mine = 0.0;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      ft = ft + 0.02;
+      mine = i == lane ? ft : mine;
+    }
+    const double ts = t_now + mine;
+    const bool in_time = ts < duration;
+    bool hit = false;
+    double radius = 0.0;
+    int k = kstart;
+    if (in_time) {
+      double pt[3];
+      deboor<3>(s.P, s.U, n, ts + s.U[3], &k, pt);
+      hit = inflate_hit(g, occ, pt);
+      const double dx = pt[0] - cur[0], dy = pt[1] - cur[1], dz = pt[2] - cur[2];
+      radius = sqrt(dx * dx + dy * dy + dz * dz);
+    }
+    const bool stop = !in_time || hit || !(radius < 6.0);
+    const unsigned bal = __ballot_sync(FULL, stop);
+    double r_prev = __shfl_up_sync(FULL, radius, 1);
+    if (lane == 0) r_prev = r_carry;
+    if (bal) {
+      const int f = __ffs(bal) - 1;
+      const bool f_in = __shfl_sync(FULL, in_time, f), f_hit = __shfl_sync(FULL, hit, f);
+      const double f_rprev = __shfl_sync(FULL, r_prev, f);
+      n_checked = base + f + (f_in ? 1 : 0);
+      if (f_in && f_hit) {
+        safe = 0;
+        distance = f_rprev;
+      }
+      break;
+    }
+    if (base + 32 >= FUELGPU_CHECK_MAX_SAMPLES) {  // a scan the reference would not finish in practice
+      n_checked = base + 32;
+      break;
+    }
+    ft_base = ft;
+    r_carry = __shfl_sync(FULL, radius, 31);
+    kstart = __shfl_sync(FULL, k, 31);
+  }
+
+  if (lane == 0) {
+    double jerk = 0.0;
+    for (int i = 0; i < n - 3; ++i)
+      for (int j = 0; j < 3; ++j) jerk += s.J[i][j];
+    const double vr = mv / prm.max_vel, ar = sqrt(fabs(ma) / prm.max_acc);
+    FuelTrajReport r;
+    r.duration = duration;
+    r.jerk = jerk;
+    r.ratio = vr < ar ? ar : vr;  // std::max(max_vel / limit_vel_, sqrt(fabs(max_acc) / limit_acc_))
+    r.distance = distance;
+    r.safe = safe;
+    r.feasible = fea ? 1 : 0;
+    r.n_checked = n_checked;
+    r.reserved = 0;
+    rep[b] = r;
+  }
+}
+
+// selectBestTraj: least jerk, lowest index on ties, NaN never wins; [1] the same among safe && feasible
+__device__ __forceinline__ bool better(double j, int i, double jc, int ic) {
+  return i >= 0 && (ic < 0 || j < jc || (j == jc && i < ic));
+}
+
+__global__ void __launch_bounds__(1024) traj_best_kernel(const FuelTrajReport* __restrict__ rep, int B, int32_t* best) {
+  __shared__ double sj[2][32];
+  __shared__ int si[2][32];
+  double j0 = 0.0, j1 = 0.0;
+  int i0 = -1, i1 = -1;
+  for (int b = threadIdx.x; b < B; b += blockDim.x) {
+    const FuelTrajReport r = rep[b];
+    if (isnan(r.jerk)) continue;
+    if (better(r.jerk, b, j0, i0)) j0 = r.jerk, i0 = b;
+    if (r.safe && r.feasible && better(r.jerk, b, j1, i1)) j1 = r.jerk, i1 = b;
+  }
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    const double a0 = __shfl_xor_sync(FULL, j0, o), a1 = __shfl_xor_sync(FULL, j1, o);
+    const int b0 = __shfl_xor_sync(FULL, i0, o), b1 = __shfl_xor_sync(FULL, i1, o);
+    if (better(a0, b0, j0, i0)) j0 = a0, i0 = b0;
+    if (better(a1, b1, j1, i1)) j1 = a1, i1 = b1;
+  }
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  if (lane == 0) sj[0][w] = j0, si[0][w] = i0, sj[1][w] = j1, si[1][w] = i1;
+  __syncthreads();
+  if (w == 0) {
+    j0 = lane < nw ? sj[0][lane] : 0.0, i0 = lane < nw ? si[0][lane] : -1;
+    j1 = lane < nw ? sj[1][lane] : 0.0, i1 = lane < nw ? si[1][lane] : -1;
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+      const double a0 = __shfl_xor_sync(FULL, j0, o), a1 = __shfl_xor_sync(FULL, j1, o);
+      const int b0 = __shfl_xor_sync(FULL, i0, o), b1 = __shfl_xor_sync(FULL, i1, o);
+      if (better(a0, b0, j0, i0)) j0 = a0, i0 = b0;
+      if (better(a1, b1, j1, i1)) j1 = a1, i1 = b1;
+    }
+    if (lane == 0) best[0] = i0, best[1] = i1;
+  }
+}
+
+// evaluateDeBoorT (:73-75) of the spline or of its first / second derivative at t [B][n_t] -> out [B][n_t][3]
+__global__ void __launch_bounds__(TC_WPB * 32) traj_evaluate_kernel(int B, int n, int nvar, const double* __restrict__ x,
+                                                                    const double* __restrict__ dtv, int n_t,
+                                                                    const double* __restrict__ t, int deriv,
+                                                                    double* __restrict__ out) {
+  __shared__ SplineSmem sm[TC_WPB];
+  const int lane = threadIdx.x & 31;
+  const int b = blockIdx.x * TC_WPB + (threadIdx.x >> 5);
+  if (b >= B) return;
+  SplineSmem& s = sm[threadIdx.x >> 5];
+  load_spline(s, b, n, nvar, x, dtv, lane);
+  for (int q = lane; q < n_t; q += 32) {
+    const size_t o = (size_t)b * n_t + q;
+    const double tq = t[o];
+    double v[3];
+    int k;
+    if (deriv == 0) {
+      k = 3;
+      deboor<3>(s.P, s.U, n, tq + s.U[3], &k, v);
+    } else if (deriv == 1) {
+      k = 2;
+      deboor<2>(s.Q, s.U + 1, n - 1, tq + s.U[3], &k, v);
+    } else {
+      k = 1;
+      deboor<1>(s.R, s.U + 2, n - 2, tq + s.U[3], &k, v);
+    }
+    out[3 * o] = v[0], out[3 * o + 1] = v[1], out[3 * o + 2] = v[2];
+  }
+}
+
+}  // namespace
+
+int traj_check_impl(FuelMap* m, int B, int n_pts, int nvar, const double* x_dev, const double* dt_dev,
+                    const FuelTrajCheckParams* p, FuelTrajReport* rep_dev, int32_t* best_dev) {
+  if (B == 0) {
+    FUEL_CUDA(m, cudaMemsetAsync(best_dev, 0xff, 2 * sizeof(int32_t), m->stream));  // -1, -1
+    return 0;
+  }
+  const int grid = (B + TC_WPB - 1) / TC_WPB;
+  traj_check_kernel<<<grid, TC_WPB * 32, 0, m->stream>>>(m->g, m->occ, B, n_pts, nvar, x_dev, dt_dev, *p, rep_dev);
+  FUEL_CUDA(m, cudaGetLastError());
+  traj_best_kernel<<<1, 1024, 0, m->stream>>>(rep_dev, B, best_dev);
+  FUEL_CUDA(m, cudaGetLastError());
+  FUEL_LAUNCHES(m, 2);
+  return 0;
+}
+
+int traj_evaluate_impl(FuelMap* m, int B, int n_pts, int nvar, const double* x_dev, const double* dt_dev, int n_t,
+                       const double* t_dev, int deriv, double* out_dev) {
+  if (B == 0 || n_t == 0) return 0;
+  const int grid = (B + TC_WPB - 1) / TC_WPB;
+  traj_evaluate_kernel<<<grid, TC_WPB * 32, 0, m->stream>>>(B, n_pts, nvar, x_dev, dt_dev, n_t, t_dev, deriv, out_dev);
+  FUEL_CUDA(m, cudaGetLastError());
+  FUEL_LAUNCHES(m, 1);
+  return 0;
+}

@@ -75,7 +75,8 @@ FUELGPU_API int fuelgpu_map_synchronize(FuelMap* map);
  * flag = int8 per voxel: frontier_flag_ */
 FUELGPU_API int fuelgpu_map_device_ptrs(FuelMap* map, void** occ, void** dist, void** flag);
 /* Milliseconds spent on the device by the last call of each stage (CUDA events on the
- * handle's stream): [0] esdf_update [1] frontier_search [2] bspline batch [3] upload [4] download */
+ * handle's stream): [0] esdf_update [1] frontier_search [2] bspline batch [3] upload [4] download
+ * [5] trajectory check (fuelgpu_bspline_check_batch[_dev]) */
 FUELGPU_API int fuelgpu_map_last_timing(FuelMap* map, float ms[8]);
 /* Where the last call of each stage sat on the device timeline: start and end in milliseconds after the start of the
  * last upload (same stage indices; -1 = stage not run or no upload recorded).  Diagnostic for overlapped sequences. */
@@ -385,6 +386,49 @@ FUELGPU_API int fuelgpu_bspline_optimize_batch_dev(FuelMap* map, int32_t B, int3
                                        const FuelOptParams* params, const void* traj_dev,
                                        const FuelSolveParams* solve, void* x_dev, void* f_best_dev,
                                        void* n_eval_dev);
+
+/* ---- trajectory verdicts: NonUniformBspline checks, checkTrajCollision, selectBestTraj -----------------------
+ * Uniform cubic B-splines (setUniformBspline(ctrl, 3, dt), bspline/src/non_uniform_bspline.cpp:16-32) in the solver's
+ * layout: x [B][nvar] holds the control points of trajectory b as x[b][3*i + axis].  nvar == 3*n_pts + 1: the knot
+ * span is x[b][3*n_pts] (MINTIME, what the solver returns) and dt must be NULL; nvar == 3*n_pts: dt [B] holds it.
+ * n_pts is 4..FUELGPU_MAX_PTS.  Every output equals the reference's fp64 arithmetic bit for bit (DESIGN.md 4.6). */
+typedef struct {
+  double max_vel, max_acc; /* setPhysicalLimits(pp_.max_vel_, pp_.max_acc_), non_uniform_bspline.cpp:129-133 */
+  double t_now;            /* checkTrajCollision's t_now (planner_manager.cpp:97): seconds since the batch's start; 0 = fresh plan */
+} FuelTrajCheckParams;
+
+typedef struct {
+  double duration;   /* getTimeSum  (:267-269) */
+  double jerk;       /* getJerk     (:283-298) */
+  double ratio;      /* checkRatio  (:135-160) */
+  double distance;   /* checkTrajCollision's `distance` out-value when unsafe; -1 when safe (the reference leaves it untouched) */
+  int32_t safe;      /* checkTrajCollision's return value */
+  int32_t feasible;  /* checkFeasibility (:443-487) */
+  int32_t n_checked; /* fut_t samples the loop evaluated before it stopped */
+  int32_t reserved;
+} FuelTrajReport;
+
+/* A collision scan stops after this many samples (20 971 s of trajectory at the reference's 0.02 s step) and reports
+ * the trajectory safe; the longest scan of the solver's output (64 points, dt 5 s) is about 15 000 samples. */
+#define FUELGPU_CHECK_MAX_SAMPLES (1 << 20)
+
+/* checkTrajCollision (planner_manager.cpp:96-118) samples the spline every 0.02 s from t_now, up to 6 m from
+ * evaluateDeBoorT(t_now) or the end, and fails on the first sample whose voxel has the inflate bit (bit 2 of the
+ * resident occupancy byte, getInflateOccupancy, sdf_map.h:217-226; outside the map is not a hit).
+ * best[0] = selectBestTraj (planner_manager.cpp:476-482): index of the least jerk (ties: lowest index; NaN never wins).
+ * best[1] = the same among trajectories with safe && feasible; -1 if none.
+ * Runs on the map's main stream, so the _dev form can be enqueued straight after fuelgpu_bspline_optimize_batch_dev
+ * on its x.  Device time: slot 5 of fuelgpu_map_last_timing. */
+FUELGPU_API int fuelgpu_bspline_check_batch(FuelMap* map, int32_t B, int32_t n_pts, int32_t nvar, const double* x,
+                                            const double* dt, const FuelTrajCheckParams* params, FuelTrajReport* report,
+                                            int32_t best[2]);
+FUELGPU_API int fuelgpu_bspline_check_batch_dev(FuelMap* map, int32_t B, int32_t n_pts, int32_t nvar, const void* x_dev,
+                                                const void* dt_dev, const FuelTrajCheckParams* params, void* report_dev,
+                                                void* best_dev);
+/* evaluateDeBoorT (:73-75) of the spline (deriv 0) or of getDerivative() once / twice (deriv 1, 2; :77-106), at
+ * t [B][n_t] per trajectory (clamped to [0, duration] like the reference); out [B][n_t][3]. */
+FUELGPU_API int fuelgpu_bspline_evaluate_batch(FuelMap* map, int32_t B, int32_t n_pts, int32_t nvar, const double* x,
+                                               const double* dt, int32_t n_t, const double* t, int32_t deriv, double* out);
 
 /* ---- multi-GPU: the z-sharded ESDF update (BASELINE config 4; SURVEY 8e row 1) ---------------------------
  * Multi-GPU form of SDFMap::updateESDF3d (plan_env/src/sdf_map.cpp:152-241) over the whole map.  One process
