@@ -161,6 +161,8 @@ SIGNATURES = {
     "fuelgpu_bspline_check_batch_dev": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, C.POINTER(FuelTrajCheckParams), _vp,
                                                   _vp]),
     "fuelgpu_bspline_evaluate_batch": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _i32, _vp, _i32, _vp]),
+    "fuelgpu_bspline_parameterize_batch": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "fuelgpu_bspline_parameterize_batch_dev": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

@@ -1051,6 +1051,65 @@ int fuelgpu_bspline_evaluate_batch(FuelMap* m, int32_t B, int32_t n_pts, int32_t
   return 0;
 }
 
+static int check_param_args(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar, const void* points, const void* derivs,
+                            const void* dt, const void* x, const void* traj) {
+  if (!m) return fuel_fail(nullptr, FUELGPU_EINVAL, "null map");
+  if (B < 0) return fuel_fail(m, FUELGPU_EINVAL, "negative batch");
+  if (n_pts < 4 || n_pts > FUELGPU_MAX_PTS) return fuel_fail(m, FUELGPU_EINVAL, "n_pts must be in 4..64");
+  if (nvar != 3 * n_pts && nvar != 3 * n_pts + 1) return fuel_fail(m, FUELGPU_EINVAL, "nvar must be 3*n_pts or 3*n_pts + 1");
+  if (B > 0 && (!points || !derivs || !dt || !x || !traj)) return fuel_fail(m, FUELGPU_EINVAL, "null argument");
+  return 0;
+}
+
+int fuelgpu_bspline_parameterize_batch_dev(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar, const void* points_dev,
+                                           const void* derivs_dev, const void* dt_dev, const void* time_lb_dev, void* x_dev,
+                                           void* traj_dev) {
+  int rc = check_param_args(m, B, n_pts, nvar, points_dev, derivs_dev, dt_dev, x_dev, traj_dev);
+  if (rc) return rc;
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  tbegin(m, T_PARAM);
+  rc = traj_param_impl(m, B, n_pts, nvar, (const double*)points_dev, (const double*)derivs_dev, (const double*)dt_dev,
+                       (const double*)time_lb_dev, (double*)x_dev, (FuelTrajConst*)traj_dev);
+  tend(m, T_PARAM);
+  return rc;
+}
+
+int fuelgpu_bspline_parameterize_batch(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar, const double* points,
+                                       const double* derivs, const double* dt, const double* time_lb, double* x,
+                                       FuelTrajConst* traj) {
+  int rc = check_param_args(m, B, n_pts, nvar, points, derivs, dt, x, traj);
+  if (rc) return rc;
+  for (int32_t b = 0; b < B; ++b)  // parameterizeToBspline prints and returns on ts <= 0 (:181-184)
+    if (!(dt[b] > 0.0 && dt[b] <= 1.7976931348623157e308))
+      return fuel_fail(m, FUELGPU_EINVAL, "dt[%s%lld] must be finite and positive", "", (long long)b);
+  if (B == 0) return 0;
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  const size_t K = (size_t)n_pts - 2;
+  const size_t pb = align256(sizeof(double) * B * K * 3), gb = align256(sizeof(double) * B * 12);
+  const size_t db = align256(sizeof(double) * B), xb = align256(sizeof(double) * B * nvar);
+  rc = ensure_tc(m, pb + gb + 2 * db + xb + sizeof(FuelTrajConst) * B);
+  if (rc) return rc;
+  uint8_t* base = (uint8_t*)m->tc_buf;
+  double* d_pts = (double*)base;
+  double* d_der = (double*)(base + pb);
+  double* d_dt = (double*)(base + pb + gb);
+  double* d_tlb = time_lb ? (double*)(base + pb + gb + db) : nullptr;
+  double* d_x = (double*)(base + pb + gb + 2 * db);
+  FuelTrajConst* d_tc = (FuelTrajConst*)(base + pb + gb + 2 * db + xb);
+  FUEL_CUDA(m, cudaMemcpyAsync(d_pts, points, sizeof(double) * B * K * 3, cudaMemcpyHostToDevice, m->stream));
+  FUEL_CUDA(m, cudaMemcpyAsync(d_der, derivs, sizeof(double) * B * 12, cudaMemcpyHostToDevice, m->stream));
+  FUEL_CUDA(m, cudaMemcpyAsync(d_dt, dt, sizeof(double) * B, cudaMemcpyHostToDevice, m->stream));
+  if (time_lb) FUEL_CUDA(m, cudaMemcpyAsync(d_tlb, time_lb, sizeof(double) * B, cudaMemcpyHostToDevice, m->stream));
+  tbegin(m, T_PARAM);
+  rc = traj_param_impl(m, B, n_pts, nvar, d_pts, d_der, d_dt, d_tlb, d_x, d_tc);
+  tend(m, T_PARAM);
+  if (rc) return rc;
+  FUEL_CUDA(m, cudaMemcpyAsync(x, d_x, sizeof(double) * B * nvar, cudaMemcpyDeviceToHost, m->stream));
+  FUEL_CUDA(m, cudaMemcpyAsync(traj, d_tc, sizeof(FuelTrajConst) * B, cudaMemcpyDeviceToHost, m->stream));
+  FUEL_CUDA(m, cudaStreamSynchronize(m->stream));
+  return 0;
+}
+
 
 
 }  // extern "C"

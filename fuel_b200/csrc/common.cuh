@@ -23,7 +23,7 @@ struct Geom {
   double box_mind[3], box_maxd[3];
 };
 
-enum { T_ESDF = 0, T_FRONTIER = 1, T_BSPLINE = 2, T_UPLOAD = 3, T_DOWNLOAD = 4, T_CHECK = 5, T_COUNT = 8 };
+enum { T_ESDF = 0, T_FRONTIER = 1, T_BSPLINE = 2, T_UPLOAD = 3, T_DOWNLOAD = 4, T_CHECK = 5, T_PARAM = 6, T_COUNT = 8 };
 
 struct FrontierState;  // frontier.cu
 struct FusionState;    // fusion.cu
@@ -176,6 +176,9 @@ int traj_check_impl(FuelMap* m, int B, int n_pts, int nvar, const double* x_dev,
                     const FuelTrajCheckParams* p, FuelTrajReport* rep_dev, int32_t* best_dev);
 int traj_evaluate_impl(FuelMap* m, int B, int n_pts, int nvar, const double* x_dev, const double* dt_dev, int n_t,
                        const double* t_dev, int deriv, double* out_dev);
+// parameterizeToBspline + the constants optimize() freezes from its control points
+int traj_param_impl(FuelMap* m, int B, int n_pts, int nvar, const double* pts_dev, const double* der_dev,
+                    const double* dt_dev, const double* tlb_dev, double* x_dev, FuelTrajConst* tc_dev);
 
 // getDistWithGrad on the device (sdf_map.cpp:497-536); shared by esdf.cu and bspline.cu
 __device__ __forceinline__ double dev_get_distance(const Geom& g, const float* __restrict__ dist,

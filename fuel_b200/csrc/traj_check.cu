@@ -1,9 +1,11 @@
 // traj_check.cu -- verdicts on a batch of uniform cubic B-splines, on the map's main stream behind the solver:
 // NonUniformBspline::evaluateDeBoorT / getDerivative / getTimeSum / getJerk / checkFeasibility / checkRatio
 // (bspline/src/non_uniform_bspline.cpp), FastPlannerManager::checkTrajCollision (planner_manager.cpp:96-118) and
-// selectBestTraj (:476-482).
+// selectBestTraj (:476-482); and, ahead of the solver, parameterizeToBspline (:178-265) with the boundary states and
+// pt_dist_ that BsplineOptimizer::optimize() freezes from its result.
 //
-// Built with -fmad=false: every output equals the reference's fp64 arithmetic bit for bit.
+// Built with -fmad=false: every output equals the reference's fp64 arithmetic bit for bit (for the parameterization:
+// given the control points it returns; their least-squares solve is this file's own, see traj_param_kernel).
 //  - knots are the running sum of setUniformBspline (:16-32), u[i] = u[i-1] + dt, not i*dt;
 //  - derivative control points are (p * (P[i+1] - P[i])) / (u[i+p+1] - u[i+1]) per element (:77-86), the derivative
 //    spline keeps the parent's knots minus the first and last (:97-106);
@@ -282,6 +284,148 @@ __global__ void __launch_bounds__(TC_WPB * 32) traj_evaluate_kernel(int B, int n
   }
 }
 
+// ---- parameterizeToBspline (:178-265), degree 3, and what optimize() freezes from its control points ------------------
+struct ParamSmem {
+  SplineSmem s;
+  double Rb[FUELGPU_MAX_PTS][3];  // band of the triangular factor: Rb[i][k] = R(i, i + k)
+  double D[FUELGPU_MAX_PTS][3];   // Q^T b per axis, rows of R
+  double seg[FUELGPU_MAX_PTS];    // |P[i+1] - P[i]| for pt_dist_
+};
+
+// Row r of the system in column order (start vel, start acc, positions 0..K-1, end vel, end acc): its first column and
+// its three coefficients, with the reference's entries (1/6.0)*(1,4,1), (1/(2*ts))*(-1,0,1), (1/(ts*ts))*(1,-2,1).
+__device__ __forceinline__ int param_row(int r, int K, double ts, const double* __restrict__ pts,
+                                         const double* __restrict__ der, double w[3], double e[3]) {
+  const double to_pos = 1 / 6.0, to_vel = 1 / (2 * ts), to_acc = 1 / (ts * ts);
+  int c, src;  // src: index into der (0 start vel, 1 end vel, 2 start acc, 3 end acc), or -1 for a position
+  if (r == 0) c = 0, src = 0;
+  else if (r == 1) c = 0, src = 2;
+  else if (r < K + 2) c = r - 2, src = -1;
+  else c = K - 1, src = r == K + 2 ? 1 : 3;
+  if (src < 0) {
+    w[0] = to_pos * 1, w[1] = to_pos * 4, w[2] = to_pos * 1;
+  } else if (src == 0 || src == 1) {
+    w[0] = to_vel * -1, w[1] = to_vel * 0, w[2] = to_vel * 1;
+  } else {
+    w[0] = to_acc * 1, w[1] = to_acc * -2, w[2] = to_acc * 1;
+  }
+  const double* bsrc = src < 0 ? pts + 3 * c : der + 3 * src;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) e[a] = bsrc[a];
+  return c;
+}
+
+// One warp per trajectory.  Lane 0 solves the (K+4) x (K+2) least-squares system with Givens rotations, row by row in
+// column order, so that the triangular factor keeps the band of A (three entries per row); the three axes share the
+// rotations.  The warp then loads the returned spline with load_spline and evaluates getBoundaryStates(2, 0) with the
+// check kernels' deboor, and sums pt_dist_ in the reference's order.  A knot span that is not finite and positive
+// gives NaN in every output of its trajectory.
+__global__ void __launch_bounds__(TC_WPB * 32) traj_param_kernel(int B, int n, int nvar, const double* __restrict__ pts,
+                                                                 const double* __restrict__ der,
+                                                                 const double* __restrict__ dtv,
+                                                                 const double* __restrict__ tlb, double* x,
+                                                                 FuelTrajConst* __restrict__ tc) {
+  __shared__ ParamSmem sm[TC_WPB];
+  const int lane = threadIdx.x & 31;
+  const int b = blockIdx.x * TC_WPB + (threadIdx.x >> 5);
+  if (b >= B) return;
+  ParamSmem& q = sm[threadIdx.x >> 5];
+  const int K = n - 2;
+  const double raw = dtv[b];
+  const double dt = isfinite(raw) && raw > 0.0 ? raw : __longlong_as_double(0x7ff8000000000000ll);
+  double* xb = x + (size_t)b * nvar;
+
+  if (lane == 0) {
+    const double* pb = pts + (size_t)b * K * 3;
+    const double* db = der + (size_t)b * 12;
+    int nfill = 0;  // rows of R filled so far: rows arrive in column order, so R fills top down
+    for (int r = 0; r < K + 4; ++r) {
+      double w[3], e[3];
+      const int c = param_row(r, K, dt, pb, db, w, e);
+      for (int j = c; j < c + 3; ++j) {
+        if (j == nfill) {
+#pragma unroll
+          for (int k = 0; k < 3; ++k) q.Rb[j][k] = w[k], q.D[j][k] = e[k];
+          ++nfill;
+          break;
+        }
+        // the rotation that zeroes w[0] against R(j, j); one reciprocal square root instead of a square root and two
+        // divisions on the dependent chain (it rounds the rotation by a few ulp, far below the solve's cond(A) * eps)
+        const double rj = q.Rb[j][0], hh = rj * rj + w[0] * w[0];
+        const double inv = hh != 0.0 ? rsqrt(hh) : 0.0;
+        const double h = hh * inv;
+        const double cs = hh != 0.0 ? rj * inv : 1.0, sn = w[0] * inv;
+        const double r1 = q.Rb[j][1], r2 = q.Rb[j][2];
+        q.Rb[j][0] = h;
+        q.Rb[j][1] = cs * r1 + sn * w[1];
+        q.Rb[j][2] = cs * r2 + sn * w[2];
+        w[0] = cs * w[1] - sn * r1;
+        w[1] = cs * w[2] - sn * r2;
+        w[2] = 0.0;
+#pragma unroll
+        for (int a = 0; a < 3; ++a) {
+          const double dj = q.D[j][a];
+          q.D[j][a] = cs * dj + sn * e[a];
+          e[a] = cs * e[a] - sn * dj;
+        }
+      }
+    }
+    double x1[3] = {0.0, 0.0, 0.0}, x2[3] = {0.0, 0.0, 0.0};  // solution rows i + 1, i + 2
+    for (int i = n - 1; i >= 0; --i) {
+#pragma unroll
+      for (int a = 0; a < 3; ++a) {
+        const double v = (q.D[i][a] - q.Rb[i][1] * x1[a] - q.Rb[i][2] * x2[a]) / q.Rb[i][0];
+        xb[3 * i + a] = v;
+        x2[a] = x1[a];
+        x1[a] = v;
+      }
+    }
+    if (nvar == 3 * n + 1) xb[3 * n] = dt;
+  }
+  __syncwarp();
+  // setUniformBspline(ctrl, 3, dt) of the returned control points; with nvar == 3n, dt comes from the input array
+  load_spline(q.s, b, n, nvar, x, dtv, lane);
+  SplineSmem& s = q.s;
+  for (int i = lane; i < n - 1; i += 32) {
+    const double a0 = s.P[i + 1][0] - s.P[i][0], a1 = s.P[i + 1][1] - s.P[i][1], a2 = s.P[i + 1][2] - s.P[i][2];
+    q.seg[i] = sqrt(a0 * a0 + a1 * a1 + a2 * a2);
+  }
+  FuelTrajConst* t = tc + b;
+  uint64_t* tw = reinterpret_cast<uint64_t*>(t);
+  for (int i = lane; i < (int)(sizeof(FuelTrajConst) / 8); i += 32) tw[i] = 0;
+  __syncwarp();
+  // getBoundaryStates(2, 0) (:108-123): pos, vel, acc at t = 0 on lanes 0-2, the end position at getTimeSum() on lane 3
+  double v[3];
+  int k;
+  if (lane == 0) {
+    k = 3;
+    deboor<3>(s.P, s.U, n, 0.0 + s.U[3], &k, v);
+  } else if (lane == 1) {
+    k = 2;
+    deboor<2>(s.Q, s.U + 1, n - 1, 0.0 + s.U[3], &k, v);
+  } else if (lane == 2) {
+    k = 1;
+    deboor<1>(s.R, s.U + 2, n - 2, 0.0 + s.U[3], &k, v);
+  } else if (lane == 3) {
+    k = 3;
+    deboor<3>(s.P, s.U, n, (s.U[n] - s.U[3]) + s.U[3], &k, v);
+  }
+  if (lane < 3) {
+    for (int a = 0; a < 3; ++a) t->start[lane][a] = v[a];
+  } else if (lane == 3) {
+    for (int a = 0; a < 3; ++a) t->end[0][a] = v[a];
+  }
+  if (lane == 0) {
+    double d = 0.0;  // pt_dist_ (bspline_optimizer.cpp:136-140): sequential sum over the segments, over the point count
+    for (int i = 0; i < n - 1; ++i) d += q.seg[i];
+    t->pt_dist = d / (double)n;
+    t->knot_span = dt;
+    t->n_end = 1;
+    t->time_lb = tlb ? tlb[b] : -1.0;
+    t->view_idx = -1;
+  }
+}
+
 }  // namespace
 
 int traj_check_impl(FuelMap* m, int B, int n_pts, int nvar, const double* x_dev, const double* dt_dev,
@@ -304,6 +448,16 @@ int traj_evaluate_impl(FuelMap* m, int B, int n_pts, int nvar, const double* x_d
   if (B == 0 || n_t == 0) return 0;
   const int grid = (B + TC_WPB - 1) / TC_WPB;
   traj_evaluate_kernel<<<grid, TC_WPB * 32, 0, m->stream>>>(B, n_pts, nvar, x_dev, dt_dev, n_t, t_dev, deriv, out_dev);
+  FUEL_CUDA(m, cudaGetLastError());
+  FUEL_LAUNCHES(m, 1);
+  return 0;
+}
+
+int traj_param_impl(FuelMap* m, int B, int n_pts, int nvar, const double* pts_dev, const double* der_dev,
+                    const double* dt_dev, const double* tlb_dev, double* x_dev, FuelTrajConst* tc_dev) {
+  if (B == 0) return 0;
+  const int grid = (B + TC_WPB - 1) / TC_WPB;
+  traj_param_kernel<<<grid, TC_WPB * 32, 0, m->stream>>>(B, n_pts, nvar, pts_dev, der_dev, dt_dev, tlb_dev, x_dev, tc_dev);
   FUEL_CUDA(m, cudaGetLastError());
   FUEL_LAUNCHES(m, 1);
   return 0;

@@ -1,6 +1,8 @@
 """NonUniformBspline (bspline/src/non_uniform_bspline.cpp) for the uniform cubic splines the planner flies, and
 FastPlannerManager's checkTrajCollision / selectBestTraj (plan_manage/src/planner_manager.cpp:96-118, 476-482), over
 fuelgpu_bspline_check_batch / fuelgpu_bspline_evaluate_batch.  Every value is the reference's fp64 result bit for bit.
+parameterize_batch / NonUniformBspline.parameterizeToBspline build the solver's batch from sampled paths
+(fuelgpu_bspline_parameterize_batch); their control points come from this project's own least-squares solve.
 
 Batches use the solver's layout: x [B, nvar] with control point i at x[b, 3i:3i+3]; nvar == 3*n_pts + 1 carries the
 knot span in the last column (what BsplineOptimizer.optimizeBatch returns with MINTIME), nvar == 3*n_pts takes dt [B].
@@ -9,7 +11,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import FuelTrajCheckParams, check, lib, ptr
+from ._lib import FuelTrajCheckParams, FuelTrajConst, check, lib, ptr
 
 # one FuelTrajReport per trajectory (include/fuelgpu.h)
 REPORT_DTYPE = np.dtype([("duration", np.float64), ("jerk", np.float64), ("ratio", np.float64),
@@ -64,6 +66,32 @@ def check_batch(sdf_map, x, n_pts, dt=None, *, max_vel, max_acc, t_now=0.0):
     return rep, best
 
 
+def parameterize_batch(sdf_map, points, derivs, dt, time_lb=None, mintime=True):
+    """parameterizeToBspline (:178-265, degree 3) of B sampled paths, the getBoundaryStates(2, 0) of the result
+    (:108-123) and the pt_dist_ optimize() freezes (bspline_optimizer.cpp:136-140), on the device of `sdf_map`
+    (fuelgpu_bspline_parameterize_batch).
+    points [B, K, 3] (point_set), derivs [B, 4, 3] (start vel, end vel, start acc, end acc), dt scalar or [B],
+    time_lb scalar or [B] (None: -1).  Returns (x [B, 3(K+2) (+1 dt column when mintime)], traj_consts: a ctypes array
+    of FuelTrajConst), ready for BsplineOptimizer.optimizeBatch and check_batch."""
+    points = np.ascontiguousarray(points, dtype=np.float64)
+    derivs = np.ascontiguousarray(derivs, dtype=np.float64)
+    if points.ndim != 3 or points.shape[2] != 3:
+        raise ValueError("points must be [B, K, 3]")
+    B, K = points.shape[:2]
+    if derivs.shape != (B, 4, 3):
+        raise ValueError("derivs must be [B, 4, 3]")
+    dt = np.ascontiguousarray(np.broadcast_to(np.asarray(dt, dtype=np.float64), (B,)))
+    if time_lb is not None:
+        time_lb = np.ascontiguousarray(np.broadcast_to(np.asarray(time_lb, dtype=np.float64), (B,)))
+    n = K + 2
+    x = np.empty((B, 3 * n + (1 if mintime else 0)), dtype=np.float64)
+    tc = (FuelTrajConst * B)()
+    h = _handle(sdf_map)
+    check(lib().fuelgpu_bspline_parameterize_batch(h, B, n, x.shape[1], ptr(points), ptr(derivs), ptr(dt), ptr(time_lb),
+                                                   ptr(x), tc), h)
+    return x, tc
+
+
 class NonUniformBspline:
     """The reference's class for one uniform cubic spline (setUniformBspline(points, 3, interval), :16-32), evaluated on
     the device of `sdf_map`.  getDerivative() may be applied twice (velocity, acceleration)."""
@@ -94,6 +122,17 @@ class NonUniformBspline:
         d = NonUniformBspline(self.control_points_, 3, self.knot_span_, self.sdf_map_, self._deriv + 1)
         d.limit_vel_, d.limit_acc_ = self.limit_vel_, self.limit_acc_
         return d
+
+    @staticmethod
+    def parameterizeToBspline(ts, point_set, start_end_derivative, degree, sdf_map):
+        """parameterizeToBspline (:178-265) of one sampled path: point_set [K, 3], start_end_derivative [4, 3] (start
+        vel, end vel, start acc, end acc) -> ctrl_pts [K+2, 3]; row b of parameterize_batch"""
+        if degree != 3:
+            raise ValueError("only degree 3 (bspline_degree_ = 3 in every launch file) is supported")
+        pts = np.asarray(point_set, dtype=np.float64).reshape(1, -1, 3)
+        der = np.asarray(start_end_derivative, dtype=np.float64).reshape(1, 4, 3)
+        x, _ = parameterize_batch(sdf_map, pts, der, ts, mintime=False)
+        return x[0].reshape(-1, 3)
 
     def setPhysicalLimits(self, vel, acc):
         self.limit_vel_, self.limit_acc_ = float(vel), float(acc)

@@ -76,7 +76,8 @@ FUELGPU_API int fuelgpu_map_synchronize(FuelMap* map);
 FUELGPU_API int fuelgpu_map_device_ptrs(FuelMap* map, void** occ, void** dist, void** flag);
 /* Milliseconds spent on the device by the last call of each stage (CUDA events on the
  * handle's stream): [0] esdf_update [1] frontier_search [2] bspline batch [3] upload [4] download
- * [5] trajectory check (fuelgpu_bspline_check_batch[_dev]) */
+ * [5] trajectory check (fuelgpu_bspline_check_batch[_dev]) [6] trajectory parameterization
+ * (fuelgpu_bspline_parameterize_batch[_dev]) */
 FUELGPU_API int fuelgpu_map_last_timing(FuelMap* map, float ms[8]);
 /* Where the last call of each stage sat on the device timeline: start and end in milliseconds after the start of the
  * last upload (same stage indices; -1 = stage not run or no upload recorded).  Diagnostic for overlapped sequences. */
@@ -429,6 +430,32 @@ FUELGPU_API int fuelgpu_bspline_check_batch_dev(FuelMap* map, int32_t B, int32_t
  * t [B][n_t] per trajectory (clamped to [0, duration] like the reference); out [B][n_t][3]. */
 FUELGPU_API int fuelgpu_bspline_evaluate_batch(FuelMap* map, int32_t B, int32_t n_pts, int32_t nvar, const double* x,
                                                const double* dt, int32_t n_t, const double* t, int32_t deriv, double* out);
+
+/* ---- trajectory parameterization: the solver's batch from sampled paths ---------------------------------------------
+ * Replaces NonUniformBspline::parameterizeToBspline (bspline/src/non_uniform_bspline.cpp:178-265, degree 3), the
+ * getBoundaryStates(2, 0) that follows it (:108-123; planner_manager.cpp:308, :561) and the pt_dist_ that
+ * BsplineOptimizer::optimize() freezes (bspline_optimizer.cpp:136-140), for B trajectories of K = n_pts - 2 samples.
+ *   points [B][n_pts-2][3]  the sampled positions (point_set)
+ *   derivs [B][4][3]        start vel, end vel, start acc, end acc (start_end_derivative)
+ *   dt [B]                  ts, the knot span of the result
+ *   time_lb [B] or NULL     copied to traj[b].time_lb (NULL: -1, none)
+ * Outputs, in the solver's layout: x [B][nvar] = the n_pts control points (nvar == 3*n_pts + 1: dt in the last column);
+ * traj [B] = pt_dist, knot_span = dt, start = getBoundaryStates(2, 0) start (pos, vel, acc), end[0] = its end position
+ * (n_end = 1), time_lb, n_guide = n_waypt = 0, view_idx = -1, every other byte 0.  The control points solve the
+ * reference's (K+4) x (K+2) least-squares system (same entries, rows and right-hand sides) by Givens rotations on its
+ * band; they agree with an exact solve to about cond(A) * 1e-16 (DESIGN.md 4.7).  Given those control points, every
+ * other output equals the reference's fp64 arithmetic bit for bit.  n_pts is 4..FUELGPU_MAX_PTS.
+ * Runs on the map's main stream, so parameterize_batch_dev -> fuelgpu_bspline_optimize_batch_dev ->
+ * fuelgpu_bspline_check_batch_dev needs no host sync.  Device time: slot 6 of fuelgpu_map_last_timing.
+ * The host entry returns FUELGPU_EINVAL and writes nothing when a dt is not finite and positive (the reference prints
+ * and returns, :181-184).  The _dev entry cannot read dt before the launch: such a trajectory gets NaN in x and in its
+ * pt_dist, knot_span, start and end[0], and the other trajectories are unaffected. */
+FUELGPU_API int fuelgpu_bspline_parameterize_batch(FuelMap* map, int32_t B, int32_t n_pts, int32_t nvar,
+                                                   const double* points, const double* derivs, const double* dt,
+                                                   const double* time_lb, double* x, FuelTrajConst* traj);
+FUELGPU_API int fuelgpu_bspline_parameterize_batch_dev(FuelMap* map, int32_t B, int32_t n_pts, int32_t nvar,
+                                                       const void* points_dev, const void* derivs_dev, const void* dt_dev,
+                                                       const void* time_lb_dev, void* x_dev, void* traj_dev);
 
 /* ---- multi-GPU: the z-sharded ESDF update (BASELINE config 4; SURVEY 8e row 1) ---------------------------
  * Multi-GPU form of SDFMap::updateESDF3d (plan_env/src/sdf_map.cpp:152-241) over the whole map.  One process
