@@ -76,6 +76,11 @@ class FuelTrajCheckParams(C.Structure):
     _fields_ = [("max_vel", C.c_double), ("max_acc", C.c_double), ("t_now", C.c_double)]
 
 
+class FuelPolyParams(C.Structure):
+    _fields_ = [("max_vel", C.c_double), ("ctrl_pt_dist", C.c_double), ("min_seg_num", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
 class FuelTrajReport(C.Structure):
     _fields_ = [("duration", C.c_double), ("jerk", C.c_double), ("ratio", C.c_double), ("distance", C.c_double),
                 ("safe", C.c_int32), ("feasible", C.c_int32), ("n_checked", C.c_int32), ("reserved", C.c_int32)]
@@ -163,6 +168,10 @@ SIGNATURES = {
     "fuelgpu_bspline_evaluate_batch": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _i32, _vp, _i32, _vp]),
     "fuelgpu_bspline_parameterize_batch": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "fuelgpu_bspline_parameterize_batch_dev": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "fuelgpu_poly_waypoints_batch": (C.c_int, [_vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                               C.POINTER(FuelPolyParams), _vp, _vp, _vp, _vp]),
+    "fuelgpu_poly_waypoints_batch_dev": (C.c_int, [_vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                                   C.POINTER(FuelPolyParams), _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

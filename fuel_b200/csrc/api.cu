@@ -1111,5 +1111,109 @@ int fuelgpu_bspline_parameterize_batch(FuelMap* m, int32_t B, int32_t n_pts, int
 }
 
 
+static bool finite_pos(double v) { return v > 0.0 && v <= 1.7976931348623157e308; }
+
+static int check_poly_args(FuelMap* m, int32_t B, int32_t w_max, const void* n_wp, const void* waypts,
+                           const void* start_vel, const void* start_acc, const FuelPolyParams* p, const void* info,
+                           const void* points, const void* derivs) {
+  if (!m) return fuel_fail(nullptr, FUELGPU_EINVAL, "null map");
+  if (B < 0) return fuel_fail(m, FUELGPU_EINVAL, "negative batch");
+  if (w_max < 3) return fuel_fail(m, FUELGPU_EINVAL, "w_max must be at least 3");
+  if (!p) return fuel_fail(m, FUELGPU_EINVAL, "null params");
+  if (!finite_pos(p->max_vel)) return fuel_fail(m, FUELGPU_EINVAL, "max_vel must be finite and positive");
+  if (!finite_pos(p->ctrl_pt_dist)) return fuel_fail(m, FUELGPU_EINVAL, "ctrl_pt_dist must be finite and positive");
+  if (p->min_seg_num < 1) return fuel_fail(m, FUELGPU_EINVAL, "min_seg_num must be at least 1");
+  if (B > 0 && (!n_wp || !waypts || !start_vel || !start_acc || !info || !points || !derivs))
+    return fuel_fail(m, FUELGPU_EINVAL, "null argument");
+  return 0;
+}
+
+int fuelgpu_poly_waypoints_batch_dev(FuelMap* m, int32_t B, int32_t w_max, const void* n_wp_dev, const void* waypts_dev,
+                                     const void* start_vel_dev, const void* start_acc_dev, const void* end_vel_dev,
+                                     const void* end_acc_dev, const void* times_dev, const FuelPolyParams* p,
+                                     void* info_dev, void* coeffs_dev, void* points_dev, void* derivs_dev) {
+  int rc = check_poly_args(m, B, w_max, n_wp_dev, waypts_dev, start_vel_dev, start_acc_dev, p, info_dev, points_dev,
+                           derivs_dev);
+  if (rc) return rc;
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  tbegin(m, T_POLY);
+  rc = poly_waypoints_impl(m, B, w_max, (const int32_t*)n_wp_dev, (const double*)waypts_dev,
+                           (const double*)start_vel_dev, (const double*)start_acc_dev, (const double*)end_vel_dev,
+                           (const double*)end_acc_dev, (const double*)times_dev, p, (FuelPolyInfo*)info_dev,
+                           (double*)coeffs_dev, (double*)points_dev, (double*)derivs_dev);
+  tend(m, T_POLY);
+  return rc;
+}
+
+int fuelgpu_poly_waypoints_batch(FuelMap* m, int32_t B, int32_t w_max, const int32_t* n_wp, const double* waypts,
+                                 const double* start_vel, const double* start_acc, const double* end_vel,
+                                 const double* end_acc, const double* times, const FuelPolyParams* p,
+                                 FuelPolyInfo* info, double* coeffs, double* points, double* derivs) {
+  int rc = check_poly_args(m, B, w_max, n_wp, waypts, start_vel, start_acc, p, info, points, derivs);
+  if (rc) return rc;
+  for (int32_t b = 0; b < B; ++b) {
+    const int32_t W = n_wp[b];
+    if (W < 3 || W > FUELGPU_MAX_WAYPTS)  // W = 2: waypointsTraj writes Ct out of bounds (polynomial_traj.cpp:74-75)
+      return fuel_fail(m, FUELGPU_EINVAL, "n_wp[%s%lld] must be in 3..32", "", (long long)b);
+    if (W > w_max) return fuel_fail(m, FUELGPU_EINVAL, "n_wp[%s%lld] exceeds w_max", "", (long long)b);
+    for (int32_t i = 0; i + 1 < W; ++i) {  // the segment times, given or as planner_manager.cpp:276-278 makes them
+      double t;
+      if (times) {
+        t = times[(size_t)b * (w_max - 1) + i];
+      } else {
+        const double* q = waypts + ((size_t)b * w_max + i) * 3;
+        const double dx = q[3] - q[0], dy = q[4] - q[1], dz = q[5] - q[2];
+        t = sqrt((dx * dx + dy * dy) + dz * dz) / (p->max_vel * 0.5);
+      }
+      if (!finite_pos(t))
+        return fuel_fail(m, FUELGPU_EINVAL, "tour %s%lld has a segment time that is not finite and positive", "",
+                         (long long)b);
+    }
+  }
+  if (B == 0) return 0;
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  const size_t S1 = (size_t)w_max - 1, K = FUELGPU_MAX_PTS - 2;
+  const size_t nb = align256(sizeof(int32_t) * B), wb = align256(sizeof(double) * B * w_max * 3);
+  const size_t vb = align256(sizeof(double) * B * 3), tb = times ? align256(sizeof(double) * B * S1) : 0;
+  const size_t ib = align256(sizeof(FuelPolyInfo) * B), cb = coeffs ? align256(sizeof(double) * B * S1 * 18) : 0;
+  const size_t pb = align256(sizeof(double) * B * K * 3), db = align256(sizeof(double) * B * 12);
+  rc = ensure_tc(m, nb + wb + 4 * vb + tb + ib + cb + pb + db);
+  if (rc) return rc;
+  uint8_t* q = (uint8_t*)m->tc_buf;
+  int32_t* d_n = (int32_t*)q;
+  q += nb;
+  double* d_wp = (double*)q;
+  q += wb;
+  double* d_sv = (double*)q;
+  double* d_sa = (double*)(q + vb);
+  double* d_ev = end_vel ? (double*)(q + 2 * vb) : nullptr;
+  double* d_ea = end_acc ? (double*)(q + 3 * vb) : nullptr;
+  q += 4 * vb;
+  double* d_t = times ? (double*)q : nullptr;
+  q += tb;
+  FuelPolyInfo* d_info = (FuelPolyInfo*)q;
+  q += ib;
+  double* d_c = coeffs ? (double*)q : nullptr;
+  q += cb;
+  double* d_p = (double*)q;
+  double* d_d = (double*)(q + pb);
+  FUEL_CUDA(m, cudaMemcpyAsync(d_n, n_wp, sizeof(int32_t) * B, cudaMemcpyHostToDevice, m->stream));
+  FUEL_CUDA(m, cudaMemcpyAsync(d_wp, waypts, sizeof(double) * B * w_max * 3, cudaMemcpyHostToDevice, m->stream));
+  FUEL_CUDA(m, cudaMemcpyAsync(d_sv, start_vel, sizeof(double) * B * 3, cudaMemcpyHostToDevice, m->stream));
+  FUEL_CUDA(m, cudaMemcpyAsync(d_sa, start_acc, sizeof(double) * B * 3, cudaMemcpyHostToDevice, m->stream));
+  if (end_vel) FUEL_CUDA(m, cudaMemcpyAsync(d_ev, end_vel, sizeof(double) * B * 3, cudaMemcpyHostToDevice, m->stream));
+  if (end_acc) FUEL_CUDA(m, cudaMemcpyAsync(d_ea, end_acc, sizeof(double) * B * 3, cudaMemcpyHostToDevice, m->stream));
+  if (times) FUEL_CUDA(m, cudaMemcpyAsync(d_t, times, sizeof(double) * B * S1, cudaMemcpyHostToDevice, m->stream));
+  tbegin(m, T_POLY);
+  rc = poly_waypoints_impl(m, B, w_max, d_n, d_wp, d_sv, d_sa, d_ev, d_ea, d_t, p, d_info, d_c, d_p, d_d);
+  tend(m, T_POLY);
+  if (rc) return rc;
+  FUEL_CUDA(m, cudaMemcpyAsync(info, d_info, sizeof(FuelPolyInfo) * B, cudaMemcpyDeviceToHost, m->stream));
+  if (coeffs) FUEL_CUDA(m, cudaMemcpyAsync(coeffs, d_c, sizeof(double) * B * S1 * 18, cudaMemcpyDeviceToHost, m->stream));
+  FUEL_CUDA(m, cudaMemcpyAsync(points, d_p, sizeof(double) * B * K * 3, cudaMemcpyDeviceToHost, m->stream));
+  FUEL_CUDA(m, cudaMemcpyAsync(derivs, d_d, sizeof(double) * B * 12, cudaMemcpyDeviceToHost, m->stream));
+  FUEL_CUDA(m, cudaStreamSynchronize(m->stream));
+  return 0;
+}
 
 }  // extern "C"

@@ -23,7 +23,7 @@ struct Geom {
   double box_mind[3], box_maxd[3];
 };
 
-enum { T_ESDF = 0, T_FRONTIER = 1, T_BSPLINE = 2, T_UPLOAD = 3, T_DOWNLOAD = 4, T_CHECK = 5, T_PARAM = 6, T_COUNT = 8 };
+enum { T_ESDF = 0, T_FRONTIER = 1, T_BSPLINE = 2, T_UPLOAD = 3, T_DOWNLOAD = 4, T_CHECK = 5, T_PARAM = 6, T_POLY = 7, T_COUNT = 8 };
 
 struct FrontierState;  // frontier.cu
 struct FusionState;    // fusion.cu
@@ -179,6 +179,11 @@ int traj_evaluate_impl(FuelMap* m, int B, int n_pts, int nvar, const double* x_d
 // parameterizeToBspline + the constants optimize() freezes from its control points
 int traj_param_impl(FuelMap* m, int B, int n_pts, int nvar, const double* pts_dev, const double* der_dev,
                     const double* dt_dev, const double* tlb_dev, double* x_dev, FuelTrajConst* tc_dev);
+// poly_traj.cu: waypointsTraj + getLength + planExploreTraj's sampling (planner_manager.cpp:270-297)
+int poly_waypoints_impl(FuelMap* m, int B, int w_max, const int32_t* n_wp_dev, const double* wp_dev,
+                        const double* sv_dev, const double* sa_dev, const double* ev_dev, const double* ea_dev,
+                        const double* times_dev, const FuelPolyParams* p, FuelPolyInfo* info_dev, double* coeffs_dev,
+                        double* points_dev, double* derivs_dev);
 
 // getDistWithGrad on the device (sdf_map.cpp:497-536); shared by esdf.cu and bspline.cu
 __device__ __forceinline__ double dev_get_distance(const Geom& g, const float* __restrict__ dist,

@@ -1,0 +1,171 @@
+"""PolynomialTraj (poly_traj/include/poly_traj/polynomial_traj.h, poly_traj/src/polynomial_traj.cpp) for the minimum-jerk
+tours the exploration planner flies, and FastPlannerManager::planExploreTraj (plan_manage/src/planner_manager.cpp:266-316)
+for B candidate tours, over fuelgpu_poly_waypoints_batch and the existing parameterize / optimize / check entries.
+
+waypoints_batch runs the polynomial stage: segment times, waypointsTraj, getTotalTime, getLength, seg_num, dt, and the
+samples and boundary derivatives parameterizeToBspline takes.  plan_explore_traj_batch chains it with
+parameterize_batch -> BsplineOptimizer.optimizeBatch -> check_batch, one launch per point count.
+"""
+import ctypes as C
+
+import numpy as np
+
+from ._lib import FuelPolyParams, check, lib, ptr
+from .non_uniform_bspline import REPORT_DTYPE, _handle, check_batch, parameterize_batch
+
+MAX_WAYPTS = 32  # FUELGPU_MAX_WAYPTS
+MAX_PTS = 64     # FUELGPU_MAX_PTS
+OK, TOO_LONG, BAD_INPUT = 0, 1, 2  # FuelPolyInfo.status
+
+# one FuelPolyInfo per tour (include/fuelgpu.h)
+INFO_DTYPE = np.dtype([("duration", np.float64), ("length", np.float64), ("dt", np.float64), ("seg_num", np.int32),
+                       ("n_pts", np.int32), ("status", np.int32), ("reserved", np.int32)])
+
+
+def _pack(tours, B, name):
+    if tours is None:
+        return None
+    a = np.ascontiguousarray(np.broadcast_to(np.asarray(tours, dtype=np.float64), (B, 3)))
+    if a.shape != (B, 3):
+        raise ValueError("%s must be [B, 3]" % name)
+    return a
+
+
+def waypoints_batch(sdf_map, tours, start_vel, start_acc, end_vel=None, end_acc=None, times=None, *, max_vel=2.0,
+                    ctrl_pt_dist=0.35, min_seg_num=8, with_coeffs=True):
+    """planExploreTraj's lines 270-297 for B tours on the device of `sdf_map` (fuelgpu_poly_waypoints_batch).
+    tours: a list of [W_b, 3] arrays (3 <= W_b <= 32); start_vel / start_acc / end_vel / end_acc: [3] or [B, 3] (end
+    None: zero); times: None (|dp| / (max_vel * 0.5)) or a list of [W_b - 1] arrays.
+    Returns (info [B] of INFO_DTYPE, coeffs [B, w_max - 1, 3, 6] or None, points [B, 62, 3], derivs [B, 4, 3]):
+    points[b, :info['n_pts'][b] - 2] are the samples, derivs[b] = start vel, end vel, start acc, end acc."""
+    tours = [np.asarray(t, dtype=np.float64).reshape(-1, 3) for t in tours]
+    B = len(tours)
+    n_wp = np.array([len(t) for t in tours], dtype=np.int32)
+    w_max = max(3, int(n_wp.max()) if B else 3)
+    wp = np.zeros((B, w_max, 3))
+    for b, t in enumerate(tours):
+        wp[b, :len(t)] = t
+    tm = None
+    if times is not None:
+        tm = np.zeros((B, w_max - 1))
+        for b, t in enumerate(times):
+            t = np.asarray(t, dtype=np.float64).ravel()
+            tm[b, :len(t)] = t
+    sv, sa = _pack(start_vel, B, "start_vel"), _pack(start_acc, B, "start_acc")
+    ev, ea = _pack(end_vel, B, "end_vel"), _pack(end_acc, B, "end_acc")
+    prm = FuelPolyParams(float(max_vel), float(ctrl_pt_dist), int(min_seg_num), 0)
+    info = np.empty(B, dtype=INFO_DTYPE)
+    coeffs = np.empty((B, w_max - 1, 3, 6)) if with_coeffs else None
+    points = np.empty((B, MAX_PTS - 2, 3))
+    derivs = np.empty((B, 4, 3))
+    h = _handle(sdf_map)
+    check(lib().fuelgpu_poly_waypoints_batch(h, B, w_max, ptr(n_wp), ptr(wp), ptr(sv), ptr(sa), ptr(ev), ptr(ea),
+                                             ptr(tm), C.byref(prm), ptr(info), ptr(coeffs), ptr(points), ptr(derivs)), h)
+    return info, coeffs, points, derivs
+
+
+class PolynomialTraj:
+    """The reference's class for one trajectory, its coefficients solved on the device of `sdf_map`.  evaluate() runs on
+    the host with the reference's segment search and Polynomial::evaluate (pow and a written-order dot)."""
+
+    def __init__(self, sdf_map):
+        self.sdf_map = sdf_map
+        self.reset()
+
+    def reset(self):
+        self.coeffs_ = np.zeros((0, 3, 6))
+        self.times_ = np.zeros(0)
+        self.info_ = None
+
+    @staticmethod
+    def waypointsTraj(positions, start_vel, end_vel, start_acc, end_acc, times, poly_traj):
+        """waypointsTraj (polynomial_traj.cpp:5-175), the reference's argument order: positions [W, 3], times [W - 1]"""
+        positions = np.asarray(positions, dtype=np.float64).reshape(-1, 3)
+        times = np.asarray(times, dtype=np.float64).ravel()
+        info, coeffs, _, _ = waypoints_batch(poly_traj.sdf_map, [positions], start_vel, start_acc, end_vel, end_acc,
+                                             [times])
+        S = len(positions) - 1
+        poly_traj.coeffs_ = coeffs[0, :S].copy()
+        poly_traj.times_ = times.copy()
+        poly_traj.info_ = info[0]
+
+    def getTotalTime(self):
+        s = 0.0
+        for t in self.times_:
+            s += float(t)
+        return s
+
+    def evaluate(self, t, k):
+        """PolynomialTraj::evaluate(t, k) (polynomial_traj.h:83-91)"""
+        idx, ts = 0, float(t)
+        while idx < len(self.times_) - 1 and self.times_[idx] + 1e-4 < ts:
+            ts -= self.times_[idx]
+            idx += 1
+        tv = np.zeros(6)
+        for i in range(k, 6):
+            coeff = 1
+            for j in range(i, i - k, -1):
+                coeff *= j
+            tv[i] = coeff * ts ** (i - k)
+        out = np.empty(3)
+        for j in range(3):
+            v = tv[0] * self.coeffs_[idx, j, 0]
+            for i in range(1, 6):
+                v = v + tv[i] * self.coeffs_[idx, j, i]
+            out[j] = v
+        return out
+
+    def getLength(self):
+        """getLength (polynomial_traj.h:107-124), as the device computed it in waypointsTraj"""
+        return float(self.info_["length"])
+
+
+def plan_explore_traj_batch(sdf_map, tours, cur_vel, cur_acc, time_lb, opt, solve, limits, *, ctrl_pt_dist=0.35,
+                            min_seg_num=8):
+    """planExploreTraj (planner_manager.cpp:266-316) for B candidate tours, then selectBestTraj (:476-482) over them.
+    opt: a BsplineOptimizer set up on `sdf_map` (its cost_function with or without MINTIME); solve: keyword arguments of
+    optimizeBatch besides x / traj_consts / n_pts (cost_function, max_eval, ...); limits: dict(max_vel=, max_acc=), the
+    pp_.max_vel_ that also sets the segment times.
+    The polynomial stage runs first; its info (B x 40 bytes) is read back, because the solver takes one point count per
+    launch.  Each group of equal n_pts then runs parameterize -> optimize -> check.  Tours with status != 0 are left
+    out and keep NaN reports.
+    Returns dict(info, x: a list of [nvar] arrays or None per tour, report [B] of REPORT_DTYPE, best [2]): best[0] =
+    least jerk (lowest index on ties, NaN never wins), best[1] = the same among safe and feasible tours, -1 if none."""
+    B = len(tours)
+    info, _, points, derivs = waypoints_batch(sdf_map, tours, cur_vel, cur_acc, max_vel=limits["max_vel"],
+                                              ctrl_pt_dist=ctrl_pt_dist, min_seg_num=min_seg_num, with_coeffs=False)
+    mask = int(solve["cost_function"])
+    mintime = bool(mask & opt.MINTIME)
+    tlb = np.broadcast_to(np.asarray(time_lb, dtype=np.float64), (B,))
+    report = np.zeros(B, dtype=REPORT_DTYPE)
+    for f in ("duration", "jerk", "ratio", "distance"):
+        report[f] = np.nan
+    xs = [None] * B
+    ok = info["status"] == OK
+    for n in sorted(set(info["n_pts"][ok].tolist())):
+        idx = np.flatnonzero(ok & (info["n_pts"] == n))
+        K = n - 2
+        x0, tc = parameterize_batch(sdf_map, points[idx, :K], derivs[idx], info["dt"][idx], time_lb=tlb[idx],
+                                    mintime=mintime)
+        kw = {k: v for k, v in solve.items() if k != "cost_function"}
+        x, _, _ = opt.optimizeBatch(x0, tc, n, mask, **kw)
+        dt = None if mintime else info["dt"][idx]
+        rep, _ = check_batch(sdf_map, x, n, dt, max_vel=limits["max_vel"], max_acc=limits["max_acc"])
+        report[idx] = rep
+        for r, b in enumerate(idx):
+            xs[b] = x[r].copy()
+    return dict(info=info, x=xs, report=report, best=select_best(report))
+
+
+def select_best(report):
+    """selectBestTraj's rule over merged reports: least jerk, lowest index on ties, NaN never wins; [1] among the safe
+    and feasible, -1 if none"""
+    best = [-1, -1]
+    for i, r in enumerate(report):
+        j = r["jerk"]
+        if not j == j:
+            continue
+        for s, ok in ((0, True), (1, bool(r["safe"]) and bool(r["feasible"]))):
+            if ok and (best[s] < 0 or j < report[best[s]]["jerk"]):
+                best[s] = i
+    return np.array(best, dtype=np.int32)

@@ -113,13 +113,13 @@ class SDFMap:
     def last_timing(self):
         ms = (C.c_float * 8)()
         check(lib().fuelgpu_map_last_timing(self._h, ms), self._h)
-        return dict(esdf=ms[0], frontier=ms[1], bspline=ms[2], upload=ms[3], download=ms[4], check=ms[5], param=ms[6])
+        return dict(esdf=ms[0], frontier=ms[1], bspline=ms[2], upload=ms[3], download=ms[4], check=ms[5], param=ms[6], poly=ms[7])
 
     def last_timeline(self):
         """(start, end) in ms after the start of the last upload, per stage."""
         t0, t1 = (C.c_float * 8)(), (C.c_float * 8)()
         check(lib().fuelgpu_map_last_timeline(self._h, t0, t1), self._h)
-        names = ("esdf", "frontier", "bspline", "upload", "download", "check", "param")
+        names = ("esdf", "frontier", "bspline", "upload", "download", "check", "param", "poly")
         return {k: (t0[i], t1[i]) for i, k in enumerate(names)}
 
     def launch_count(self):

@@ -274,3 +274,54 @@ def depth_frame(g, inflate, cam_pos, yaw, pitch=0.0, width=640, height=480, fx=3
     dirs_c = np.stack([(U - cx) / fx, (V - cy) / fy, np.ones_like(U, dtype=np.float64)], axis=-1).reshape(-1, 3)
     pts = (dirs_c * d[:, None]) @ R.T + np.asarray(cam_pos, dtype=np.float64)
     return np.ascontiguousarray(pts[keep], dtype=np.float32)
+
+
+def make_tours(g, inflate, B=1024, seed=20261015, spacing=3.0, max_vel=2.0, max_acc=2.0):
+    """Candidate tours for planExploreTraj, shaped like shortenPath's output (fast_exploration_manager.cpp:239-263,
+    321-323): 3 to 12 waypoints about `spacing` apart in the free space of the exploration box, a short midpoint
+    inserted into the first leg of some of them (always into a one-leg tour, as shortenPath does).  Most tours are 1.5 to
+    8 m long, so their point counts span several groups from 11 up; about 4 % are 13 to 18 m (n_pts up to about 64), and the
+    last tour is about 30 m (past FUELGPU_MAX_PTS).  Start velocity / acceleration are random within max_vel / max_acc.
+    Returns dict(tours: list of [W, 3] arrays, start_vel [B, 3], start_acc [B, 3])."""
+    rng = np.random.default_rng(seed)
+    lo = g.box_min + 0.15
+    hi = g.box_max - 0.15
+
+    def free(p):
+        if np.any(p < lo) or np.any(p > hi):
+            return False
+        i = g.pos_to_index(p)
+        return not inflate[i[0], i[1], i[2]]
+
+    tours = []
+    while len(tours) < B:
+        last = len(tours) == B - 1
+        r = rng.uniform()
+        L = 30.0 if last else (rng.uniform(13.0, 18.0) if r < 0.04 else rng.uniform(1.5, 8.0))
+        n_leg = int(min(11, max(1, round(L / spacing))))
+        p = rng.uniform(lo, hi)
+        if not free(p):
+            continue
+        pts = [p]
+        for _ in range(n_leg):
+            for _try in range(20):
+                d = rng.normal(size=3)
+                d[2] *= 0.15
+                q = pts[-1] + d / np.linalg.norm(d) * (L / n_leg) * rng.uniform(0.85, 1.15)
+                if free(q):
+                    pts.append(q)
+                    break
+            else:
+                break
+        if len(pts) != n_leg + 1:
+            continue
+        if n_leg == 1 or rng.uniform() < 0.2:
+            pts.insert(1, 0.5 * (pts[0] + pts[1]))
+        tours.append(np.array(pts))
+    dirs = rng.normal(size=(B, 3))
+    dirs /= np.linalg.norm(dirs, axis=1, keepdims=True)
+    start_vel = dirs * rng.uniform(0.0, max_vel, (B, 1))
+    dirs = rng.normal(size=(B, 3))
+    dirs /= np.linalg.norm(dirs, axis=1, keepdims=True)
+    start_acc = dirs * rng.uniform(0.0, max_acc, (B, 1))
+    return dict(tours=tours, start_vel=start_vel, start_acc=start_acc)

@@ -77,7 +77,7 @@ FUELGPU_API int fuelgpu_map_device_ptrs(FuelMap* map, void** occ, void** dist, v
 /* Milliseconds spent on the device by the last call of each stage (CUDA events on the
  * handle's stream): [0] esdf_update [1] frontier_search [2] bspline batch [3] upload [4] download
  * [5] trajectory check (fuelgpu_bspline_check_batch[_dev]) [6] trajectory parameterization
- * (fuelgpu_bspline_parameterize_batch[_dev]) */
+ * (fuelgpu_bspline_parameterize_batch[_dev]) [7] waypoint polynomial (fuelgpu_poly_waypoints_batch[_dev]) */
 FUELGPU_API int fuelgpu_map_last_timing(FuelMap* map, float ms[8]);
 /* Where the last call of each stage sat on the device timeline: start and end in milliseconds after the start of the
  * last upload (same stage indices; -1 = stage not run or no upload recorded).  Diagnostic for overlapped sequences. */
@@ -456,6 +456,64 @@ FUELGPU_API int fuelgpu_bspline_parameterize_batch(FuelMap* map, int32_t B, int3
 FUELGPU_API int fuelgpu_bspline_parameterize_batch_dev(FuelMap* map, int32_t B, int32_t n_pts, int32_t nvar,
                                                        const void* points_dev, const void* derivs_dev, const void* dt_dev,
                                                        const void* time_lb_dev, void* x_dev, void* traj_dev);
+
+/* ---- waypoint polynomial: the head of planExploreTraj on the device ---------------------------------------------------
+ * Replaces FastPlannerManager::planExploreTraj's lines 270-297 (plan_manage/src/planner_manager.cpp) for B tours: the
+ * segment times (:276-278), PolynomialTraj::waypointsTraj (poly_traj/src/polynomial_traj.cpp:5-175), getTotalTime and
+ * getLength (polynomial_traj.h:83-124), seg_num = max(min_seg_num, (int)(length / ctrl_pt_dist)), dt = duration /
+ * seg_num (:285-288), the samples at ts = 0, dt, ... while ts <= duration + 1e-4 and the four boundary derivatives
+ * (:292-297), laid out as the input of fuelgpu_bspline_parameterize_batch.
+ *   n_wp [B]                      waypoints of tour b, 3..FUELGPU_MAX_WAYPTS (S = n_wp - 1 segments)
+ *   waypts [B][w_max][3]          the tours, padded to w_max rows
+ *   start_vel, start_acc [B][3]   cur_vel, cur_acc
+ *   end_vel, end_acc [B][3]       or NULL: zero, what planExploreTraj passes
+ *   times [B][w_max-1]            segment times, or NULL: |p[i+1] - p[i]| / (max_vel * 0.5), the norm taken as
+ *                                 sqrt((dx*dx + dy*dy) + dz*dz) (Eigen's order is unpinned)
+ * Outputs: info [B]; coeffs [B][w_max-1][3][6] or NULL (segment k, axis j: cx[i] multiplies t^i, as
+ * Polynomial(cx, cy, cz, T) stores it; rows >= S zero); points [B][FUELGPU_MAX_PTS-2][3] (the K = n_pts - 2 samples,
+ * rows >= K zero); derivs [B][4][3] (start vel, end vel, start acc, end acc).
+ * The coefficients solve the reference's minimum-jerk problem without its dense inverses (a block-tridiagonal LDL^T in
+ * the inner velocities and accelerations, DESIGN.md 4.8); they agree with an exact solve to
+ * within 1e-11 relative on the test grid (S up to 31, times 0.05 to 5 s).
+ * duration, dt, the sample times, K and the times computed from the waypoints equal the reference's fp64 arithmetic
+ * bit for bit; length, the samples and derivs agree to rounding, and so seg_num does except where length /
+ * ctrl_pt_dist lies within rounding of an integer.  A tour whose n_pts would exceed FUELGPU_MAX_PTS gets status
+ * FUELGPU_POLY_TOO_LONG, its info and coefficients, zero points and its derivs.
+ * Tours of two waypoints are refused: the reference's waypointsTraj writes Ct(3, 2S+4) and Ct(5, 2S+5) there, columns 6
+ * and 7 of a 6-column matrix; shortenPath (fast_exploration_manager.cpp:321-323) never hands it such a tour.
+ * Runs on the map's main stream, so fuelgpu_poly_waypoints_batch_dev -> fuelgpu_bspline_parameterize_batch_dev -> ...
+ * needs no host sync except to read info[].n_pts.  Device time: slot 7 of fuelgpu_map_last_timing.
+ * The host entry returns FUELGPU_EINVAL and writes nothing when an n_wp is outside 3..FUELGPU_MAX_WAYPTS or above w_max,
+ * a segment time (given or computed) is not finite and positive (a repeated waypoint makes A singular), max_vel or
+ * ctrl_pt_dist is not finite and positive, or min_seg_num < 1.  The _dev entry checks the parameters alone; a tour with
+ * a bad n_wp or time gets status FUELGPU_POLY_BAD_INPUT, NaN in every double it outputs and seg_num = n_pts = 0, and the
+ * other tours are unaffected. */
+#define FUELGPU_MAX_WAYPTS 32
+#define FUELGPU_POLY_TOO_LONG 1
+#define FUELGPU_POLY_BAD_INPUT 2
+typedef struct {
+  double max_vel;      /* pp_.max_vel_: times = |p[i+1]-p[i]| / (max_vel*0.5) when times == NULL (planner_manager.cpp:276-278) */
+  double ctrl_pt_dist; /* pp_.ctrl_pt_dist (manager/control_points_distance, 0.35 in algorithm.xml) */
+  int32_t min_seg_num; /* 8 in planExploreTraj (:287) */
+  int32_t reserved;
+} FuelPolyParams;
+typedef struct {
+  double duration, length, dt; /* getTotalTime, getLength, duration / seg_num */
+  int32_t seg_num, n_pts;      /* n_pts = K + 2: the point count to hand to parameterize / optimize / check */
+  int32_t status;              /* 0, FUELGPU_POLY_TOO_LONG (n_pts > FUELGPU_MAX_PTS), FUELGPU_POLY_BAD_INPUT (_dev only) */
+  int32_t reserved;
+} FuelPolyInfo;
+FUELGPU_API int fuelgpu_poly_waypoints_batch(FuelMap* map, int32_t B, int32_t w_max, const int32_t* n_wp,
+                                             const double* waypts, const double* start_vel, const double* start_acc,
+                                             const double* end_vel, const double* end_acc, const double* times,
+                                             const FuelPolyParams* params, FuelPolyInfo* info, double* coeffs,
+                                             double* points, double* derivs);
+FUELGPU_API int fuelgpu_poly_waypoints_batch_dev(FuelMap* map, int32_t B, int32_t w_max, const void* n_wp_dev,
+                                                 const void* waypts_dev, const void* start_vel_dev,
+                                                 const void* start_acc_dev, const void* end_vel_dev,
+                                                 const void* end_acc_dev, const void* times_dev,
+                                                 const FuelPolyParams* params, void* info_dev, void* coeffs_dev,
+                                                 void* points_dev, void* derivs_dev);
 
 /* ---- multi-GPU: the z-sharded ESDF update (BASELINE config 4; SURVEY 8e row 1) ---------------------------
  * Multi-GPU form of SDFMap::updateESDF3d (plan_env/src/sdf_map.cpp:152-241) over the whole map.  One process
