@@ -81,6 +81,14 @@ class FuelPolyParams(C.Structure):
                 ("reserved", C.c_int32)]
 
 
+class FuelYawParams(C.Structure):
+    _fields_ = [("relax_time", C.c_double), ("lookfwd", C.c_int32), ("reserved", C.c_int32)]
+
+
+class FuelYawInfo(C.Structure):
+    _fields_ = [("dt_yaw", C.c_double), ("pt_dist", C.c_double), ("n_waypt", C.c_int32), ("status", C.c_int32)]
+
+
 class FuelTrajReport(C.Structure):
     _fields_ = [("duration", C.c_double), ("jerk", C.c_double), ("ratio", C.c_double), ("distance", C.c_double),
                 ("safe", C.c_int32), ("feasible", C.c_int32), ("n_checked", C.c_int32), ("reserved", C.c_int32)]
@@ -172,6 +180,10 @@ SIGNATURES = {
                                                C.POINTER(FuelPolyParams), _vp, _vp, _vp, _vp]),
     "fuelgpu_poly_waypoints_batch_dev": (C.c_int, [_vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                                    C.POINTER(FuelPolyParams), _vp, _vp, _vp, _vp]),
+    "fuelgpu_yaw_explore_batch": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, C.POINTER(FuelOptParams),
+                                            C.POINTER(FuelYawParams), _vp, _vp, _vp]),
+    "fuelgpu_yaw_explore_batch_dev": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, C.POINTER(FuelOptParams),
+                                                C.POINTER(FuelYawParams), _vp, _vp, _vp]),
 }
 
 _lib = None

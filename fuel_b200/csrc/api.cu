@@ -1216,4 +1216,76 @@ int fuelgpu_poly_waypoints_batch(FuelMap* m, int32_t B, int32_t w_max, const int
   return 0;
 }
 
+static int check_yaw_args(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar, const void* x, const void* dt,
+                          const void* start_yaw, const void* end_yaw, const FuelOptParams* p, const FuelYawParams* yp,
+                          const void* yaw, const void* info) {
+  int rc = check_traj_args(m, B, n_pts, nvar, x != nullptr, dt != nullptr);
+  if (rc) return rc;
+  if (!p || !yp) return fuel_fail(m, FUELGPU_EINVAL, "null params");
+  if (!finite_pos(p->ld_smooth) || !finite_pos(p->ld_start))
+    return fuel_fail(m, FUELGPU_EINVAL, "ld_smooth and ld_start must be finite and positive");
+  if (!(yp->relax_time >= 0.0 && yp->relax_time <= 1.7976931348623157e308))
+    return fuel_fail(m, FUELGPU_EINVAL, "relax_time must be finite and >= 0");
+  if (B > 0 && (!start_yaw || !end_yaw || !yaw || !info)) return fuel_fail(m, FUELGPU_EINVAL, "null argument");
+  return 0;
+}
+
+int fuelgpu_yaw_explore_batch_dev(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar, const void* x_dev,
+                                  const void* dt_dev, const void* start_yaw_dev, const void* end_yaw_dev,
+                                  const FuelOptParams* p, const FuelYawParams* yp, void* yaw_dev, void* info_dev,
+                                  void* waypt_dev) {
+  int rc = check_yaw_args(m, B, n_pts, nvar, x_dev, dt_dev, start_yaw_dev, end_yaw_dev, p, yp, yaw_dev, info_dev);
+  if (rc) return rc;
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  return yaw_explore_impl(m, B, n_pts, nvar, (const double*)x_dev, (const double*)dt_dev, (const double*)start_yaw_dev,
+                          (const double*)end_yaw_dev, p, yp, (double*)yaw_dev, (FuelYawInfo*)info_dev,
+                          (double*)waypt_dev);
+}
+
+int fuelgpu_yaw_explore_batch(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar, const double* x, const double* dt,
+                              const double* start_yaw, const double* end_yaw, const FuelOptParams* p,
+                              const FuelYawParams* yp, double* yaw, FuelYawInfo* info, double* waypt) {
+  int rc = check_yaw_args(m, B, n_pts, nvar, x, dt, start_yaw, end_yaw, p, yp, yaw, info);
+  if (rc) return rc;
+  for (int32_t b = 0; b < B; ++b) {
+    const double d = dt ? dt[b] : x[(size_t)b * nvar + 3 * n_pts];
+    if (!finite_pos(d)) return fuel_fail(m, FUELGPU_EINVAL, "dt of trajectory %s%lld must be finite and positive", "",
+                                         (long long)b);
+    const double* s = start_yaw + 3 * (size_t)b;
+    // the reference's wrapping loops (planner_manager.cpp:782-783) never end on a non-finite start yaw
+    if (!(fabs(s[0]) <= FUELGPU_YAW_MAX_START) || !isfinite(s[1]) || !isfinite(s[2]) || !isfinite(end_yaw[b]))
+      return fuel_fail(m, FUELGPU_EINVAL, "trajectory %s%lld: start yaw must be finite with |yaw| <= 1000, end yaw finite",
+                       "", (long long)b);
+  }
+  if (B == 0) return 0;
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  const size_t xb = align256(sizeof(double) * B * nvar), db = align256(sizeof(double) * B);
+  const size_t sb = align256(sizeof(double) * B * 3), yb = align256(sizeof(double) * B * FUELGPU_YAW_PTS);
+  const size_t ib = align256(sizeof(FuelYawInfo) * B), wb = sizeof(double) * B * FUELGPU_YAW_MAX_WAYPT;
+  rc = ensure_tc(m, xb + 2 * db + sb + yb + ib + wb);
+  if (rc) return rc;
+  uint8_t* q = (uint8_t*)m->tc_buf;
+  double* d_x = (double*)q;
+  double* d_dt = dt ? (double*)(q + xb) : nullptr;
+  double* d_ey = (double*)(q + xb + db);
+  q += xb + 2 * db;
+  double* d_sy = (double*)q;
+  double* d_yaw = (double*)(q + sb);
+  FuelYawInfo* d_info = (FuelYawInfo*)(q + sb + yb);
+  double* d_wp = waypt ? (double*)(q + sb + yb + ib) : nullptr;
+  FUEL_CUDA(m, cudaMemcpyAsync(d_x, x, sizeof(double) * B * nvar, cudaMemcpyHostToDevice, m->stream));
+  if (dt) FUEL_CUDA(m, cudaMemcpyAsync(d_dt, dt, sizeof(double) * B, cudaMemcpyHostToDevice, m->stream));
+  FUEL_CUDA(m, cudaMemcpyAsync(d_sy, start_yaw, sizeof(double) * B * 3, cudaMemcpyHostToDevice, m->stream));
+  FUEL_CUDA(m, cudaMemcpyAsync(d_ey, end_yaw, sizeof(double) * B, cudaMemcpyHostToDevice, m->stream));
+  rc = yaw_explore_impl(m, B, n_pts, nvar, d_x, d_dt, d_sy, d_ey, p, yp, d_yaw, d_info, d_wp);
+  if (rc) return rc;
+  FUEL_CUDA(m, cudaMemcpyAsync(yaw, d_yaw, sizeof(double) * B * FUELGPU_YAW_PTS, cudaMemcpyDeviceToHost, m->stream));
+  FUEL_CUDA(m, cudaMemcpyAsync(info, d_info, sizeof(FuelYawInfo) * B, cudaMemcpyDeviceToHost, m->stream));
+  if (waypt)
+    FUEL_CUDA(m, cudaMemcpyAsync(waypt, d_wp, sizeof(double) * B * FUELGPU_YAW_MAX_WAYPT, cudaMemcpyDeviceToHost,
+                                 m->stream));
+  FUEL_CUDA(m, cudaStreamSynchronize(m->stream));
+  return 0;
+}
+
 }  // extern "C"

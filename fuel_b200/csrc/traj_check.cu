@@ -426,6 +426,209 @@ __global__ void __launch_bounds__(TC_WPB * 32) traj_param_kernel(int B, int n, i
   }
 }
 
+// ---- planYawExplore (planner_manager.cpp:774-865) with lookfwd, on each trajectory of the batch -----------------------
+constexpr int YS = FUELGPU_YAW_SEG_NUM, YP = FUELGPU_YAW_PTS, YW = FUELGPU_YAW_MAX_WAYPT;
+constexpr double YAW_PI = 3.141592653589793;  // M_PI
+
+struct YawSmem {
+  SplineSmem s;
+  double wp[YW];     // atan2 of look-ahead difference i + 1 (NaN where |pd| <= 1e-6), then waypoint i + 1
+  double Hb[YP][4];  // normal equations, Hb[i][d] = H(i, i - d); the Cholesky factor in place
+  double r[YP];      // right-hand side, then the solution
+};
+
+// calcNextYaw (:867-885)
+__device__ __forceinline__ double next_yaw(double last_yaw, double yaw) {
+  double round_last = last_yaw;
+  while (round_last < -YAW_PI) round_last += 2 * YAW_PI;
+  while (round_last > YAW_PI) round_last -= 2 * YAW_PI;
+  const double diff = yaw - round_last;
+  if (fabs(diff) <= YAW_PI) return last_yaw + diff;
+  if (diff > YAW_PI) return last_yaw + diff - 2 * YAW_PI;
+  return last_yaw + diff + 2 * YAW_PI;
+}
+
+// w * (a . q - t)^2 over control points o .. o + L - 1, added to H and r (the objective's Hessian and gradient at 0,
+// both halved)
+template <int L>
+__device__ __forceinline__ void yaw_term(YawSmem& y, int o, const double (&a)[L], double w, double t) {
+#pragma unroll
+  for (int u = 0; u < L; ++u) {
+#pragma unroll
+    for (int v = 0; v <= u; ++v) y.Hb[o + u][u - v] += (w * a[u]) * a[v];
+    y.r[o + u] += (w * a[u]) * t;
+  }
+}
+
+// One warp per trajectory.  Lanes 0..10 evaluate the look-ahead differences of waypoints 1..11 with the check kernels'
+// deboor; lane 0 then chains calcNextYaw in the reference's order, builds the initial guess and pt_dist_, assembles the
+// normal equations of combineCost's SMOOTHNESS | START | END | WAYPOINTS terms (dim_ == 1) and solves them by banded
+// Cholesky.  Each term is stored as w * (a . q - t)^2 with integer a: 1/6 (1, 4, 1) becomes (1, 4, 1) over w / 36 and
+// 6 t, 1/(2 dt) (-1, 0, 1) becomes (-1, 0, 1) over w / (4 dt^2) and 2 dt t, 1/dt^2 (1, -2, 1) likewise.
+__global__ void __launch_bounds__(TC_WPB * 32) yaw_explore_kernel(int B, int n, int nvar, const double* __restrict__ x,
+                                                                  const double* __restrict__ dtv,
+                                                                  const double* __restrict__ syaw,
+                                                                  const double* __restrict__ eyaw, FuelOptParams prm,
+                                                                  FuelYawParams yprm, double* __restrict__ yaw,
+                                                                  FuelYawInfo* __restrict__ info,
+                                                                  double* __restrict__ wpt) {
+  __shared__ YawSmem sm[TC_WPB];
+  const int lane = threadIdx.x & 31;
+  const int b = blockIdx.x * TC_WPB + (threadIdx.x >> 5);
+  if (b >= B) return;
+  YawSmem& y = sm[threadIdx.x >> 5];
+  const double nan = __longlong_as_double(0x7ff8000000000000ll);
+
+  const double dt = nvar == 3 * n + 1 ? x[(size_t)b * nvar + 3 * n] : dtv[b];
+  double y0 = syaw[3 * b];
+  const double y1 = syaw[3 * b + 1], y2 = syaw[3 * b + 2];
+  double ye = eyaw[b];
+  bool bad = !(dt > 0.0 && dt <= 1.7976931348623157e308) || !isfinite(y1) || !isfinite(y2) || !isfinite(ye) ||
+             !(fabs(y0) <= FUELGPU_YAW_MAX_START);
+  double dt_yaw = nan, duration = nan;
+  if (!bad) {
+    load_spline(y.s, b, n, nvar, x, dtv, lane);
+    duration = y.s.U[n] - y.s.U[3];  // getTimeSum
+    dt_yaw = duration / YS;
+    bad = !(dt_yaw > 0.0 && dt_yaw <= 1.7976931348623157e308);
+  }
+  int status = 0, nw = 0;
+  if (bad) {
+    status = FUELGPU_YAW_BAD_INPUT;
+    dt_yaw = nan;
+  } else if (yprm.lookfwd) {
+    // (int)(relax_time / dt_yaw): any quotient >= 11 leaves no waypoint; from 2^31 on the conversion is undefined
+    const double qr = yprm.relax_time / dt_yaw;
+    if (qr >= 2147483648.0) status = FUELGPU_YAW_RELAX_OVERFLOW;
+    else nw = qr >= (double)YW ? 0 : YW - (int)qr;
+  }
+  // waypoint i = l + 1: lane l evaluates pc at tc, lane l + 16 pf at min(duration, tc + forward_t)
+  const int l = lane & 15;
+  double p[3] = {0.0, 0.0, 0.0};
+  if (l < nw) {
+    const double tc = (double)(l + 1) * dt_yaw;
+    const double tf2 = tc + 2.0;
+    const double t = lane < 16 ? tc : tf2 < duration ? tf2 : duration;
+    int k = 3;
+    deboor<3>(y.s.P, y.s.U, n, t + y.s.U[3], &k, p);
+  }
+  const double dx = __shfl_down_sync(FULL, p[0], 16) - p[0], dy = __shfl_down_sync(FULL, p[1], 16) - p[1],
+               dz = __shfl_down_sync(FULL, p[2], 16) - p[2];
+  if (lane < nw) y.wp[lane] = sqrt((dx * dx + dy * dy) + dz * dz) > 1e-6 ? atan2(dy, dx) : nan;
+  __syncwarp();
+  if (lane != 0) return;
+
+  // the start wrap (|y0| <= FUELGPU_YAW_MAX_START bounds it) and the calcNextYaw chain (:782-821)
+  if (!bad) {
+    while (y0 < -YAW_PI) y0 += 2 * YAW_PI;
+    while (y0 > YAW_PI) y0 -= 2 * YAW_PI;
+  }
+  double last_yaw = y0;
+  for (int i = 0; i < nw; ++i) {
+    double w = y.wp[i];
+    if (w != w) {  // waypt = waypts.back()
+      if (i == 0) {
+        status = FUELGPU_YAW_NO_LOOKAHEAD;
+        break;
+      }
+      w = y.wp[i - 1];
+    } else {
+      w = next_yaw(last_yaw, w);
+    }
+    last_yaw = w;
+    y.wp[i] = w;
+  }
+  double pt_dist = nan;
+  if (status == 0) {
+    ye = next_yaw(last_yaw, ye);
+    // the initial guess: states2pts * start_yaw3d in rows 0-2, states2pts * (end, 0, 0) in rows 12-14
+    const double c13 = ((1 / 3.0) * dt_yaw) * dt_yaw, c16 = ((-(1 / 6.0)) * dt_yaw) * dt_yaw;
+    double g[YP];
+#pragma unroll
+    for (int i = 0; i < YP; ++i) g[i] = 0.0;
+    g[0] = (1.0 * y0 + -dt_yaw * y1) + c13 * y2;
+    g[1] = (1.0 * y0 + 0.0 * y1) + c16 * y2;
+    g[2] = (1.0 * y0 + dt_yaw * y1) + c13 * y2;
+    g[YS] = (1.0 * ye + -dt_yaw * 0.0) + c13 * 0.0;
+    g[YS + 1] = (1.0 * ye + 0.0 * 0.0) + c16 * 0.0;
+    g[YS + 2] = (1.0 * ye + dt_yaw * 0.0) + c13 * 0.0;
+    double d = 0.0;  // pt_dist_ (bspline_optimizer.cpp:136-140): |row(i + 1) - row(i)| of a one-column matrix
+#pragma unroll
+    for (int i = 0; i < YP - 1; ++i) {
+      const double e = g[i + 1] - g[i];
+      d += sqrt(e * e);
+    }
+    pt_dist = d / (double)YP;
+    if (pt_dist == 0.0) status = FUELGPU_YAW_ZERO_PT_DIST;
+  }
+
+  if (status == 0) {
+#pragma unroll
+    for (int i = 0; i < YP; ++i) {
+      y.r[i] = 0.0;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) y.Hb[i][k] = 0.0;
+    }
+    const double jerk[4] = {-1.0, 3.0, -3.0, 1.0}, pos[3] = {1.0, 4.0, 1.0}, vel[3] = {-1.0, 0.0, 1.0},
+                 acc[3] = {1.0, -2.0, 1.0};
+    const double ws = prm.ld_smooth / (pt_dist * pt_dist), dt2 = dt_yaw * dt_yaw;
+    for (int i = 0; i + 3 < YP; ++i) yaw_term<4>(y, i, jerk, ws, 0.0);
+    yaw_term<3>(y, 0, pos, prm.ld_start * 10.0 / 36.0, 6.0 * y0);
+    yaw_term<3>(y, 0, vel, prm.ld_start / (4.0 * dt2), 2.0 * dt_yaw * y1);
+    yaw_term<3>(y, 0, acc, prm.ld_start / (dt2 * dt2), dt2 * y2);
+    yaw_term<3>(y, YS, pos, prm.ld_end / 36.0, 6.0 * ye);
+    yaw_term<3>(y, YS, vel, prm.ld_end / (4.0 * dt2), 0.0);
+    for (int i = 0; i < nw; ++i) yaw_term<3>(y, i + 1, pos, prm.ld_waypt / 36.0, 6.0 * y.wp[i]);
+    // banded Cholesky H = L L^T, L(i, k) in Hb[i][i - k]
+    for (int j = 0; j < YP && status == 0; ++j) {
+      double dj = y.Hb[j][0];
+      for (int k = j < 3 ? 0 : j - 3; k < j; ++k) dj -= y.Hb[j][j - k] * y.Hb[j][j - k];
+      if (!(dj > 0.0 && dj <= 1.7976931348623157e308)) {
+        status = FUELGPU_YAW_NOT_SPD;
+        break;
+      }
+      const double ljj = sqrt(dj);
+      y.Hb[j][0] = ljj;
+      for (int i = j + 1; i <= j + 3 && i < YP; ++i) {
+        double s = y.Hb[i][i - j];
+        for (int k = i - 3; k < j; ++k)
+          if (k >= 0) s -= y.Hb[i][i - k] * y.Hb[j][j - k];
+        y.Hb[i][i - j] = s / ljj;
+      }
+    }
+    if (status == 0) {
+      for (int j = 0; j < YP; ++j) {  // L z = r
+        double s = y.r[j];
+        for (int k = j < 3 ? 0 : j - 3; k < j; ++k) s -= y.Hb[j][j - k] * y.r[k];
+        y.r[j] = s / y.Hb[j][0];
+      }
+      for (int j = YP - 1; j >= 0; --j) {  // L^T q = z
+        double s = y.r[j];
+        for (int i = j + 1; i <= j + 3 && i < YP; ++i) s -= y.Hb[i][i - j] * y.r[i];
+        y.r[j] = s / y.Hb[j][0];
+      }
+      bool fin = true;
+      for (int j = 0; j < YP; ++j) fin = fin && isfinite(y.r[j]);
+      if (!fin) status = FUELGPU_YAW_NOT_SPD;
+    }
+  }
+
+  // what the reference defined before a failure is written, the rest is NaN
+  const bool have_wp = status == 0 || status == FUELGPU_YAW_ZERO_PT_DIST || status == FUELGPU_YAW_NOT_SPD;
+  double* yb = yaw + (size_t)b * YP;
+  for (int j = 0; j < YP; ++j) yb[j] = status == 0 ? y.r[j] : nan;
+  if (wpt) {
+    double* wb = wpt + (size_t)b * YW;
+    for (int i = 0; i < YW; ++i) wb[i] = !have_wp ? nan : i < nw ? y.wp[i] : 0.0;
+  }
+  FuelYawInfo o;
+  o.dt_yaw = dt_yaw;
+  o.pt_dist = have_wp ? pt_dist : nan;
+  o.n_waypt = have_wp ? nw : 0;
+  o.status = status;
+  info[b] = o;
+}
+
 }  // namespace
 
 int traj_check_impl(FuelMap* m, int B, int n_pts, int nvar, const double* x_dev, const double* dt_dev,
@@ -458,6 +661,18 @@ int traj_param_impl(FuelMap* m, int B, int n_pts, int nvar, const double* pts_de
   if (B == 0) return 0;
   const int grid = (B + TC_WPB - 1) / TC_WPB;
   traj_param_kernel<<<grid, TC_WPB * 32, 0, m->stream>>>(B, n_pts, nvar, pts_dev, der_dev, dt_dev, tlb_dev, x_dev, tc_dev);
+  FUEL_CUDA(m, cudaGetLastError());
+  FUEL_LAUNCHES(m, 1);
+  return 0;
+}
+
+int yaw_explore_impl(FuelMap* m, int B, int n_pts, int nvar, const double* x_dev, const double* dt_dev,
+                     const double* syaw_dev, const double* eyaw_dev, const FuelOptParams* p, const FuelYawParams* yp,
+                     double* yaw_dev, FuelYawInfo* info_dev, double* wpt_dev) {
+  if (B == 0) return 0;
+  const int grid = (B + TC_WPB - 1) / TC_WPB;
+  yaw_explore_kernel<<<grid, TC_WPB * 32, 0, m->stream>>>(B, n_pts, nvar, x_dev, dt_dev, syaw_dev, eyaw_dev, *p, *yp,
+                                                          yaw_dev, info_dev, wpt_dev);
   FUEL_CUDA(m, cudaGetLastError());
   FUEL_LAUNCHES(m, 1);
   return 0;

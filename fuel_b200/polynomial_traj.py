@@ -5,17 +5,23 @@ for B candidate tours, over fuelgpu_poly_waypoints_batch and the existing parame
 waypoints_batch runs the polynomial stage: segment times, waypointsTraj, getTotalTime, getLength, seg_num, dt, and the
 samples and boundary derivatives parameterizeToBspline takes.  plan_explore_traj_batch chains it with
 parameterize_batch -> BsplineOptimizer.optimizeBatch -> check_batch, one launch per point count.
+plan_yaw_explore_batch is planYawExplore (:774-865) on every trajectory of a solver batch (fuelgpu_yaw_explore_batch).
 """
 import ctypes as C
 
 import numpy as np
 
-from ._lib import FuelPolyParams, check, lib, ptr
-from .non_uniform_bspline import REPORT_DTYPE, _handle, check_batch, parameterize_batch
+from ._lib import FuelOptParams, FuelPolyParams, FuelYawParams, check, lib, ptr
+from .non_uniform_bspline import REPORT_DTYPE, _handle, _inputs, check_batch, parameterize_batch
 
 MAX_WAYPTS = 32  # FUELGPU_MAX_WAYPTS
 MAX_PTS = 64     # FUELGPU_MAX_PTS
 OK, TOO_LONG, BAD_INPUT = 0, 1, 2  # FuelPolyInfo.status
+YAW_SEG_NUM, YAW_PTS, YAW_MAX_WAYPT = 12, 15, 11  # FUELGPU_YAW_SEG_NUM, _PTS, _MAX_WAYPT
+# FuelYawInfo.status
+YAW_OK, YAW_BAD_INPUT, YAW_RELAX_OVERFLOW, YAW_NO_LOOKAHEAD, YAW_ZERO_PT_DIST, YAW_NOT_SPD = 0, 1, 2, 3, 4, 5
+YAW_INFO_DTYPE = np.dtype([("dt_yaw", np.float64), ("pt_dist", np.float64), ("n_waypt", np.int32),
+                           ("status", np.int32)])
 
 # one FuelPolyInfo per tour (include/fuelgpu.h)
 INFO_DTYPE = np.dtype([("duration", np.float64), ("length", np.float64), ("dt", np.float64), ("seg_num", np.int32),
@@ -120,8 +126,32 @@ class PolynomialTraj:
         return float(self.info_["length"])
 
 
+def plan_yaw_explore_batch(sdf_map, x, n_pts, start_yaw, end_yaw, opt_params, relax_time=1.0, lookfwd=True, dt=None):
+    """planYawExplore(start_yaw, end_yaw, lookfwd, relax_time) (planner_manager.cpp:774-865) with every trajectory of a
+    batch as the position trajectory, on the device of `sdf_map` (fuelgpu_yaw_explore_batch).
+    x: [B, nvar] in the solver's layout (dt in the last column, or dt [B] given); start_yaw: [3] or [B, 3] (yaw, yawdot,
+    yawddot); end_yaw: scalar or [B]; opt_params: a FuelOptParams or a BsplineOptimizer (ld_smooth, ld_start, ld_end and
+    ld_waypt are read).
+    Returns (yaw [B, 15] control points of the yaw spline with knot span info['dt_yaw'], info [B] of YAW_INFO_DTYPE,
+    waypt [B, 11]: the look-ahead waypoints, zero past info['n_waypt']).  A trajectory with info['status'] != 0 has NaN
+    yaw (include/fuelgpu.h lists the statuses)."""
+    x, dt = _inputs(x, n_pts, dt)
+    B = x.shape[0]
+    sy = np.ascontiguousarray(np.broadcast_to(np.asarray(start_yaw, dtype=np.float64), (B, 3)))
+    ey = np.ascontiguousarray(np.broadcast_to(np.asarray(end_yaw, dtype=np.float64), (B,)))
+    prm = opt_params if isinstance(opt_params, FuelOptParams) else opt_params.params_
+    yp = FuelYawParams(float(relax_time), 1 if lookfwd else 0, 0)
+    yaw = np.empty((B, YAW_PTS))
+    info = np.empty(B, dtype=YAW_INFO_DTYPE)
+    waypt = np.empty((B, YAW_MAX_WAYPT))
+    h = _handle(sdf_map)
+    check(lib().fuelgpu_yaw_explore_batch(h, B, n_pts, x.shape[1], ptr(x), ptr(dt), ptr(sy), ptr(ey), C.byref(prm),
+                                          C.byref(yp), ptr(yaw), ptr(info), ptr(waypt)), h)
+    return yaw, info, waypt
+
+
 def plan_explore_traj_batch(sdf_map, tours, cur_vel, cur_acc, time_lb, opt, solve, limits, *, ctrl_pt_dist=0.35,
-                            min_seg_num=8):
+                            min_seg_num=8, start_yaw=None, end_yaw=None, relax_time=1.0):
     """planExploreTraj (planner_manager.cpp:266-316) for B candidate tours, then selectBestTraj (:476-482) over them.
     opt: a BsplineOptimizer set up on `sdf_map` (its cost_function with or without MINTIME); solve: keyword arguments of
     optimizeBatch besides x / traj_consts / n_pts (cost_function, max_eval, ...); limits: dict(max_vel=, max_acc=), the
@@ -130,8 +160,21 @@ def plan_explore_traj_batch(sdf_map, tours, cur_vel, cur_acc, time_lb, opt, solv
     launch.  Each group of equal n_pts then runs parameterize -> optimize -> check.  Tours with status != 0 are left
     out and keep NaN reports.
     Returns dict(info, x: a list of [nvar] arrays or None per tour, report [B] of REPORT_DTYPE, best [2]): best[0] =
-    least jerk (lowest index on ties, NaN never wins), best[1] = the same among safe and feasible tours, -1 if none."""
+    least jerk (lowest index on ties, NaN never wins), best[1] = the same among safe and feasible tours, -1 if none.
+    With start_yaw ([3] or [B, 3]) and end_yaw (scalar or [B]) given, each group also runs planYawExplore on its solver
+    output (plan_yaw_explore_batch with lookfwd and relax_time), and the dict gains yaw [B, 15] and yaw_info [B] of
+    YAW_INFO_DTYPE (NaN and status -1 for tours left out)."""
     B = len(tours)
+    with_yaw = start_yaw is not None or end_yaw is not None
+    if with_yaw:
+        if start_yaw is None or end_yaw is None:
+            raise ValueError("start_yaw and end_yaw go together")
+        sy = np.broadcast_to(np.asarray(start_yaw, dtype=np.float64), (B, 3))
+        ey = np.broadcast_to(np.asarray(end_yaw, dtype=np.float64), (B,))
+        yaw = np.full((B, YAW_PTS), np.nan)
+        yaw_info = np.zeros(B, dtype=YAW_INFO_DTYPE)
+        yaw_info["dt_yaw"] = yaw_info["pt_dist"] = np.nan
+        yaw_info["status"] = -1
     info, _, points, derivs = waypoints_batch(sdf_map, tours, cur_vel, cur_acc, max_vel=limits["max_vel"],
                                               ctrl_pt_dist=ctrl_pt_dist, min_seg_num=min_seg_num, with_coeffs=False)
     mask = int(solve["cost_function"])
@@ -154,7 +197,13 @@ def plan_explore_traj_batch(sdf_map, tours, cur_vel, cur_acc, time_lb, opt, solv
         report[idx] = rep
         for r, b in enumerate(idx):
             xs[b] = x[r].copy()
-    return dict(info=info, x=xs, report=report, best=select_best(report))
+        if with_yaw:
+            yaw[idx], yaw_info[idx], _ = plan_yaw_explore_batch(sdf_map, x, n, sy[idx], ey[idx], opt.params_,
+                                                                relax_time=relax_time, dt=dt)
+    out = dict(info=info, x=xs, report=report, best=select_best(report))
+    if with_yaw:
+        out.update(yaw=yaw, yaw_info=yaw_info)
+    return out
 
 
 def select_best(report):

@@ -325,3 +325,27 @@ def make_tours(g, inflate, B=1024, seed=20261015, spacing=3.0, max_vel=2.0, max_
     dirs /= np.linalg.norm(dirs, axis=1, keepdims=True)
     start_acc = dirs * rng.uniform(0.0, max_acc, (B, 1))
     return dict(tours=tours, start_vel=start_vel, start_acc=start_acc)
+
+
+def make_yaws(B, seed=20261016, heading=None):
+    """Start and end yaws for planYawExplore (planner_manager.cpp:774-865) over a batch of B trajectories.
+    start [B, 3] = (yaw, yawdot, yawddot): yaw uniform in [-pi, pi], a quarter of them 1 to 5 whole turns outside it
+    (the wrapping loops run); rates uniform in [-1, 1] rad/s and [-1, 1] rad/s^2.  end [B]: uniform in [-pi, pi].
+    heading [B] (optional, e.g. the direction of travel at each trajectory's end): then every fourth end yaw lies 1e-3 to
+    0.1 rad inside heading +- pi, where calcNextYaw's |diff| is close to pi.
+    Returns dict(start [B, 3], end [B])."""
+    rng = np.random.default_rng(seed)
+    start = np.empty((B, 3))
+    start[:, 0] = rng.uniform(-np.pi, np.pi, B)
+    turns = rng.integers(1, 6, B) * rng.choice([-1, 1], B)
+    outside = rng.uniform(size=B) < 0.25
+    start[outside, 0] += 2 * np.pi * turns[outside]
+    start[:, 1] = rng.uniform(-1.0, 1.0, B)
+    start[:, 2] = rng.uniform(-1.0, 1.0, B)
+    end = rng.uniform(-np.pi, np.pi, B)
+    if heading is not None:
+        h = np.broadcast_to(np.asarray(heading, dtype=np.float64), (B,))
+        near = np.arange(B) % 4 == 3
+        side = rng.choice([-1.0, 1.0], B)
+        end[near] = h[near] + side[near] * (np.pi - rng.uniform(1e-3, 0.1, B)[near])
+    return dict(start=start, end=end)

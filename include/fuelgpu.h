@@ -515,6 +515,65 @@ FUELGPU_API int fuelgpu_poly_waypoints_batch_dev(FuelMap* map, int32_t B, int32_
                                                  const FuelPolyParams* params, void* info_dev, void* coeffs_dev,
                                                  void* points_dev, void* derivs_dev);
 
+/* ---- exploration yaw: planYawExplore on the device ----------------------------------------------------------------------
+ * Replaces FastPlannerManager::planYawExplore(start_yaw, end_yaw, lookfwd, relax_time) (plan_manage/src/
+ * planner_manager.cpp:774-865, calcNextYaw :867-885) for every trajectory of a batch in the solver's layout (x [B][nvar]
+ * with n_pts 4..FUELGPU_MAX_PTS, dt in the last column when nvar == 3*n_pts + 1, else dt [B]; see the trajectory
+ * verdicts above).  Per trajectory: dt_yaw = getTimeSum() / FUELGPU_YAW_SEG_NUM; the start yaw wrapped into [-pi, pi];
+ * the look-ahead waypoints atan2 of evaluateDeBoorT(min(duration, tc + 2)) - evaluateDeBoorT(tc) at tc = i * dt_yaw,
+ * i = 1 .. 11 - (int)(relax_time / dt_yaw), chained through calcNextYaw; the 15 x 1 initial guess and pt_dist_ that
+ * BsplineOptimizer::optimize() freezes from it; and the minimizer of its SMOOTHNESS | START | END | WAYPOINTS objective
+ * (combineCost with dim_ == 1, bspline_optimizer.cpp:518-630).  That objective is a strictly convex quadratic: the device
+ * solves its normal equations (half-bandwidth 3) by a banded Cholesky factorization in fp64 instead of running NLopt
+ * (DESIGN.md 4.9).  dt_yaw and the waypoint count equal the reference's fp64 arithmetic bit for bit; the waypoints agree
+ * to atan2's rounding (2 ulp), and given them so do the end yaw, the initial guess and pt_dist.
+ *   start_yaw [B][3]   yaw, yawdot, yawddot (finite, |yaw| <= 1000: this library's bound on the reference's wrapping loops)
+ *   end_yaw [B]        finite
+ *   params             ld_smooth, ld_start, ld_end and ld_waypt are read (ld_smooth and ld_start finite and > 0)
+ *   yaw_params         relax_time (finite, >= 0) and lookfwd (0: no waypoints)
+ * Outputs: yaw [B][FUELGPU_YAW_PTS] (the yaw control points, knot span info[b].dt_yaw); info [B]; waypt
+ * [B][FUELGPU_YAW_MAX_WAYPT] or NULL (waypoint k constrains control points k+1..k+3; zero past n_waypt).
+ * Where the reference's behaviour is undefined a trajectory gets a status and NaN yaw.  What the reference computed
+ * before that point is written (dt_yaw always; pt_dist, n_waypt and the waypoints for FUELGPU_YAW_ZERO_PT_DIST and
+ * FUELGPU_YAW_NOT_SPD), the rest is NaN, n_waypt 0:
+ *   FUELGPU_YAW_BAD_INPUT       (_dev only) a dt, start yaw or end yaw the host entry refuses, or dt_yaw not finite and > 0
+ *   FUELGPU_YAW_RELAX_OVERFLOW  relax_time / dt_yaw >= 2^31: the reference's int conversion is undefined
+ *   FUELGPU_YAW_NO_LOOKAHEAD    the first look-ahead difference is <= 1e-6 m: the reference reads waypts.back() of an
+ *                               empty vector
+ *   FUELGPU_YAW_ZERO_PT_DIST    pt_dist_ == 0 (all start and end states 0): every cost of the reference is NaN
+ *   FUELGPU_YAW_NOT_SPD         a non-positive or non-finite pivot in the factorization
+ * Runs on the map's main stream, so fuelgpu_bspline_check_batch_dev -> fuelgpu_yaw_explore_batch_dev needs no host sync.
+ * The host entry returns FUELGPU_EINVAL and writes nothing on a bad n_pts or nvar, B < 0, a dt that is not finite and
+ * positive, a bad start or end yaw, or a bad parameter; the _dev entry checks the parameters alone and marks a bad
+ * trajectory FUELGPU_YAW_BAD_INPUT, leaving the others unaffected.  Not timed in fuelgpu_map_last_timing. */
+#define FUELGPU_YAW_SEG_NUM 12
+#define FUELGPU_YAW_PTS (FUELGPU_YAW_SEG_NUM + 3)
+#define FUELGPU_YAW_MAX_WAYPT (FUELGPU_YAW_SEG_NUM - 1)
+#define FUELGPU_YAW_MAX_START 1000.0
+#define FUELGPU_YAW_BAD_INPUT 1
+#define FUELGPU_YAW_RELAX_OVERFLOW 2
+#define FUELGPU_YAW_NO_LOOKAHEAD 3
+#define FUELGPU_YAW_ZERO_PT_DIST 4
+#define FUELGPU_YAW_NOT_SPD 5
+typedef struct {
+  double relax_time; /* ep_->relax_time_ (exploration_manager/launch/algorithm.xml: 1.0) */
+  int32_t lookfwd;   /* planYawExplore's lookfwd; planExploreMotion passes true */
+  int32_t reserved;
+} FuelYawParams;
+typedef struct {
+  double dt_yaw, pt_dist; /* knot span of the yaw spline; pt_dist_ of the initial guess */
+  int32_t n_waypt;        /* look-ahead waypoints, 0..FUELGPU_YAW_MAX_WAYPT */
+  int32_t status;         /* 0 or FUELGPU_YAW_* */
+} FuelYawInfo;
+FUELGPU_API int fuelgpu_yaw_explore_batch(FuelMap* map, int32_t B, int32_t n_pts, int32_t nvar, const double* x,
+                                          const double* dt, const double* start_yaw, const double* end_yaw,
+                                          const FuelOptParams* params, const FuelYawParams* yaw_params, double* yaw,
+                                          FuelYawInfo* info, double* waypt);
+FUELGPU_API int fuelgpu_yaw_explore_batch_dev(FuelMap* map, int32_t B, int32_t n_pts, int32_t nvar, const void* x_dev,
+                                              const void* dt_dev, const void* start_yaw_dev, const void* end_yaw_dev,
+                                              const FuelOptParams* params, const FuelYawParams* yaw_params,
+                                              void* yaw_dev, void* info_dev, void* waypt_dev);
+
 /* ---- multi-GPU: the z-sharded ESDF update (BASELINE config 4; SURVEY 8e row 1) ---------------------------
  * Multi-GPU form of SDFMap::updateESDF3d (plan_env/src/sdf_map.cpp:152-241) over the whole map.  One process
  * (or thread) per GPU; rank r owns planes [r*nz/G, (r+1)*nz/G) of every (x,y) column, z fastest like the
