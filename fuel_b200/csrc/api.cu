@@ -239,7 +239,7 @@ int fuelgpu_map_destroy(FuelMap* m) {
   for (int i = 0; i < 2; ++i)
     if (m->esdf_ev[i]) cudaEventDestroy(m->esdf_ev[i]);
   void* ptrs[] = { m->occ,       m->dist,      m->dist_neg, m->flag,   m->esdf_rec,
-                   m->esdf_p[0], m->esdf_p[1], m->stage,    m->bs_buf, m->fr_scr, m->bs_grad, m->tc_buf };
+                   m->esdf_p[0], m->esdf_p[1], m->stage,    m->bs_buf, m->fr_scr, m->bs_grad, m->tc_buf, m->as_buf };
   for (void* p : ptrs)
     if (p) cudaFree(p);
   for (int t = 0; t < T_COUNT; ++t) {
@@ -1284,6 +1284,72 @@ int fuelgpu_yaw_explore_batch(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar
   if (waypt)
     FUEL_CUDA(m, cudaMemcpyAsync(waypt, d_wp, sizeof(double) * B * FUELGPU_YAW_MAX_WAYPT, cudaMemcpyDeviceToHost,
                                  m->stream));
+  FUEL_CUDA(m, cudaStreamSynchronize(m->stream));
+  return 0;
+}
+
+static int check_astar_args(FuelMap* m, int32_t B, const void* start, const void* goal, const FuelAstarParams* p,
+                            const void* info, int32_t path_max, const void* path, int32_t w_max, const void* n_wp,
+                            const void* waypts) {
+  if (!m) return fuel_fail(nullptr, FUELGPU_EINVAL, "null map");
+  if (B < 0) return fuel_fail(m, FUELGPU_EINVAL, "negative batch");
+  if (!p) return fuel_fail(m, FUELGPU_EINVAL, "null params");
+  // above 1e-3 the reference's neighbour loop (astar2.cpp:90-94) makes exactly the 26 steps
+  if (!(p->resolution > 1e-3 && p->resolution <= 1.7976931348623157e308))
+    return fuel_fail(m, FUELGPU_EINVAL, "resolution must be finite and > 1e-3");
+  if (!isfinite(p->lambda_heu)) return fuel_fail(m, FUELGPU_EINVAL, "lambda_heu must be finite");
+  if (p->allocate_num < 2 || p->max_iter < 1)
+    return fuel_fail(m, FUELGPU_EINVAL, "allocate_num must be at least 2 and max_iter at least 1");
+  if (p->allocate_num > (1 << 28)) return fuel_fail(m, FUELGPU_EINVAL, "allocate_num above 2^28");
+  if (w_max < 3) return fuel_fail(m, FUELGPU_EINVAL, "w_max must be at least 3");
+  if (path && path_max < 1) return fuel_fail(m, FUELGPU_EINVAL, "path_max must be at least 1 with a path buffer");
+  if (B > 0 && (!start || !goal || !info || !n_wp || !waypts)) return fuel_fail(m, FUELGPU_EINVAL, "null argument");
+  return 0;
+}
+
+int fuelgpu_astar_batch_dev(FuelMap* m, int32_t B, const void* start_dev, const void* goal_dev, const FuelAstarParams* p,
+                            void* info_dev, int32_t path_max, void* path_dev, int32_t w_max, void* n_wp_dev,
+                            void* waypts_dev) {
+  int rc = check_astar_args(m, B, start_dev, goal_dev, p, info_dev, path_max, path_dev, w_max, n_wp_dev, waypts_dev);
+  if (rc) return rc;
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  return astar_impl(m, B, (const double*)start_dev, (const double*)goal_dev, p, (FuelPathInfo*)info_dev, path_max,
+                    (double*)path_dev, w_max, (int32_t*)n_wp_dev, (double*)waypts_dev);
+}
+
+int fuelgpu_astar_batch(FuelMap* m, int32_t B, const double* start, const double* goal, const FuelAstarParams* p,
+                        FuelPathInfo* info, int32_t path_max, double* path, int32_t w_max, int32_t* n_wp,
+                        double* waypts) {
+  int rc = check_astar_args(m, B, start, goal, p, info, path_max, path, w_max, n_wp, waypts);
+  if (rc) return rc;
+  for (int32_t b = 0; b < B; ++b)
+    for (int k = 0; k < 3; ++k)
+      if (!isfinite(start[3 * (size_t)b + k]) || !isfinite(goal[3 * (size_t)b + k]))
+        return fuel_fail(m, FUELGPU_EINVAL, "query %s%lld: start and goal must be finite", "", (long long)b);
+  if (B == 0) return 0;
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  const size_t vb = align256(sizeof(double) * B * 3), ib = align256(sizeof(FuelPathInfo) * B);
+  const size_t pb = path ? align256(sizeof(double) * B * (size_t)path_max * 3) : 0;
+  const size_t nb = align256(sizeof(int32_t) * B), wb = sizeof(double) * B * (size_t)w_max * 3;
+  rc = ensure_tc(m, 2 * vb + ib + pb + nb + wb);
+  if (rc) return rc;
+  uint8_t* q = (uint8_t*)m->tc_buf;
+  double* d_s = (double*)q;
+  double* d_g = (double*)(q + vb);
+  FuelPathInfo* d_info = (FuelPathInfo*)(q + 2 * vb);
+  double* d_path = path ? (double*)(q + 2 * vb + ib) : nullptr;
+  int32_t* d_n = (int32_t*)(q + 2 * vb + ib + pb);
+  double* d_wp = (double*)(q + 2 * vb + ib + pb + nb);
+  FUEL_CUDA(m, cudaMemcpyAsync(d_s, start, sizeof(double) * B * 3, cudaMemcpyHostToDevice, m->stream));
+  FUEL_CUDA(m, cudaMemcpyAsync(d_g, goal, sizeof(double) * B * 3, cudaMemcpyHostToDevice, m->stream));
+  rc = astar_impl(m, B, d_s, d_g, p, d_info, path_max, d_path, w_max, d_n, d_wp);
+  if (rc) return rc;
+  FUEL_CUDA(m, cudaMemcpyAsync(info, d_info, sizeof(FuelPathInfo) * B, cudaMemcpyDeviceToHost, m->stream));
+  if (path)
+    FUEL_CUDA(m, cudaMemcpyAsync(path, d_path, sizeof(double) * B * (size_t)path_max * 3, cudaMemcpyDeviceToHost,
+                                 m->stream));
+  FUEL_CUDA(m, cudaMemcpyAsync(n_wp, d_n, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, m->stream));
+  FUEL_CUDA(m, cudaMemcpyAsync(waypts, d_wp, wb, cudaMemcpyDeviceToHost, m->stream));
   FUEL_CUDA(m, cudaStreamSynchronize(m->stream));
   return 0;
 }

@@ -73,6 +73,9 @@ struct FuelMap {
   char err[512];
   void* tc_buf;  // device scratch of the host-facing trajectory check / evaluate calls, grown on demand
   size_t tc_bytes;
+  void* as_buf;  // A* search scratch (astar.cu), grown on demand
+  size_t as_bytes;
+  size_t as_stride, as_warps;  // layout whose key tables are known empty: per-warp bytes, warps
 };
 
 extern thread_local char g_fuelgpu_err[512];
@@ -188,6 +191,9 @@ int poly_waypoints_impl(FuelMap* m, int B, int w_max, const int32_t* n_wp_dev, c
                         const double* sv_dev, const double* sa_dev, const double* ev_dev, const double* ea_dev,
                         const double* times_dev, const FuelPolyParams* p, FuelPolyInfo* info_dev, double* coeffs_dev,
                         double* points_dev, double* derivs_dev);
+// astar.cu: Astar::search + shortenPath + planExploreMotion's goal branch (fast_exploration_manager.cpp:238-263)
+int astar_impl(FuelMap* m, int B, const double* start_dev, const double* goal_dev, const FuelAstarParams* p,
+               FuelPathInfo* info_dev, int path_max, double* path_dev, int w_max, int32_t* nwp_dev, double* wp_dev);
 
 // getDistWithGrad on the device (sdf_map.cpp:497-536); shared by esdf.cu and bspline.cu
 __device__ __forceinline__ double dev_get_distance(const Geom& g, const float* __restrict__ dist,

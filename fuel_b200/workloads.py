@@ -349,3 +349,79 @@ def make_yaws(B, seed=20261016, heading=None):
         side = rng.choice([-1.0, 1.0], B)
         end[near] = h[near] + side[near] * (np.pi - rng.uniform(1e-3, 0.1, B)[near])
     return dict(start=start, end=end)
+
+
+def make_path_queries(g, inflate, tri, B=1024, seed=20261017):
+    """Start / goal pairs for Astar::search as planExploreMotion issues them (fast_exploration_manager.cpp:238-241).
+    Starts lie in known-free space inside the exploration box (tri = office_known's).  Goals, in turn: a candidate
+    viewpoint of a frontier cluster (a point 1.5 to 2.5 m from a known-free voxel next to unknown space, in the
+    sampleViewpoints ring, known-free itself); a known-free point 0.3 to 20 m away; a goal inside unknown, occupied
+    (inflated) or enclosed space; and, rarely, start == goal or a goal one voxel away.
+    Returns dict(start [B, 3], goal [B, 3], kind [B]: 0 viewpoint, 1 free, 2 unknown, 3 occupied, 4 same, 5 adjacent)."""
+    rng = np.random.default_rng(seed)
+    lo = g.box_min + 0.15
+    hi = g.box_max - 0.15
+    free = (np.asarray(tri) == FREE) & (np.asarray(inflate) == 0)
+    fidx = np.argwhere(free)
+    fpos = g.index_to_pos(fidx)
+    inb = np.all((fpos > lo) & (fpos < hi), axis=1)
+    fidx, fpos = fidx[inb], fpos[inb]
+    unk = np.asarray(tri) == UNKNOWN
+    # known-free voxels with an unknown 6-neighbour: where frontier clusters sit
+    edge = np.zeros_like(free)
+    for a in range(3):
+        for s in (-1, 1):
+            edge |= np.roll(unk, s, axis=a)
+    fr = free & edge
+    fr_idx = np.argwhere(fr)
+    fr_pos = g.index_to_pos(fr_idx)
+    fr_pos = fr_pos[np.all((fr_pos > lo) & (fr_pos < hi), axis=1)]
+    occ_pos = g.index_to_pos(np.argwhere(np.asarray(inflate) == 1))
+    occ_pos = occ_pos[np.all((occ_pos > lo) & (occ_pos < hi), axis=1)]
+    unk_pos = g.index_to_pos(np.argwhere(unk))
+    unk_pos = unk_pos[np.all((unk_pos > lo) & (unk_pos < hi), axis=1)]
+    fset = set(map(tuple, fidx.tolist()))
+
+    def is_free(p):
+        if np.any(p <= lo) or np.any(p >= hi):
+            return False
+        return tuple(g.pos_to_index(p).tolist()) in fset
+
+    start = np.empty((B, 3))
+    goal = np.empty((B, 3))
+    kind = np.empty(B, np.int32)
+    b = 0
+    while b < B:
+        s = fpos[rng.integers(len(fpos))] + rng.uniform(-0.04, 0.04, 3)
+        if not is_free(s):
+            continue
+        r = rng.uniform()
+        if r < 0.45:
+            k = 0
+            c = fr_pos[rng.integers(len(fr_pos))]
+            phi = rng.uniform(-np.pi, np.pi)
+            q = c + rng.uniform(1.5, 2.5) * np.array([np.cos(phi), np.sin(phi), 0.0])
+            if not is_free(q):
+                continue
+        elif r < 0.80:
+            k = 1
+            d = rng.normal(size=3)
+            d[2] *= 0.2
+            q = s + d / np.linalg.norm(d) * rng.uniform(0.3, 20.0)
+            if not is_free(q):
+                continue
+        elif r < 0.88:
+            k = 2
+            q = unk_pos[rng.integers(len(unk_pos))] + rng.uniform(-0.04, 0.04, 3)
+        elif r < 0.96:
+            k = 3
+            q = occ_pos[rng.integers(len(occ_pos))] + rng.uniform(-0.04, 0.04, 3)
+        elif r < 0.98:
+            k = 4
+            q = s.copy()
+        else:
+            k = 5
+            q = s + rng.choice([-1.0, 0.0, 1.0], 3) * g.res
+        start[b], goal[b], kind[b] = s, q, k
+        b += 1
+    return dict(start=start, goal=goal, kind=kind)

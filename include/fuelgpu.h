@@ -574,6 +574,78 @@ FUELGPU_API int fuelgpu_yaw_explore_batch_dev(FuelMap* map, int32_t B, int32_t n
                                               const FuelOptParams* params, const FuelYawParams* yaw_params,
                                               void* yaw_dev, void* info_dev, void* waypt_dev);
 
+/* ---- geometric path to the next viewpoint: Astar::search, shortenPath and the goal branch on the device -------------
+ * Replaces, for B (start, goal) queries, the head of FastExplorationManager::planExploreMotion
+ * (exploration_manager/src/fast_exploration_manager.cpp:238-263): path_finder_->reset(), Astar::search(pos, next_pos)
+ * (path_searching/src/astar2.cpp:47-149) with getPath / backtrack (:177-190), shortenPath (:295-325, dist_thresh 3.0,
+ * its ray test the RayCaster walk of the viewpoint visibility), Astar::pathLength (:169-175) and the radius_close = 1.5 /
+ * radius_far = 5.0 branch with the far-goal truncation (:253-262).  Every search reads the resident occupancy byte (the
+ * inflate bit and the tri-state) with the reference's tests: isInBox, getInflateOccupancy == 1 || getOccupancy ==
+ * UNKNOWN, the check points every 0.1 m along each step; A* nodes are keyed by floor((p - origin) / resolution) on the
+ * map's origin.  The open set is libstdc++'s std::priority_queue restated over node ids (its stale, re-pushed entries
+ * included), so every output equals the reference's fp64 arithmetic bit for bit (DESIGN.md 4.10).
+ *   start, goal [B][3]   pos and next_pos (finite)
+ *   params               resolution (finite and > 1e-3: the reference's neighbour loop then has its 26 steps),
+ *                        lambda_heu (finite), allocate_num (>= 2: the node pool), max_iter (>= 1)
+ * The reference's wall-clock cut (max_search_time_) is replaced by an iteration cap: the search ends with NO_PATH at
+ * loop iteration max_iter + 1, with early_terminate_cost = g + getDiagHeu(pos, end) of the open set's top.  The open
+ * set holds at most 2 * allocate_num entries on the device (the reference's is unbounded): a push beyond that ends the
+ * search with NO_PATH and reason FUELGPU_ASTAR_HEAP_FULL, never silently.
+ * Outputs: info [B]; path [B][path_max][3] or NULL: getPath() (start ... end node, goal), its first path_max rows, zero
+ * past them; waypts [B][w_max][3] and n_wp [B]: the tour planExploreTraj receives (the shortened path for CLOSE and
+ * MID, the truncated one for FAR), exactly the input of fuelgpu_poly_waypoints_batch[_dev].  n_wp[b] is the tour's
+ * count when tour_status is 0 and 0 otherwise (no path, a tour of fewer than 3 points -- start == goal hands
+ * planExploreTraj a single point -- or one longer than FUELGPU_MAX_WAYPTS or w_max); the poly entry's _dev form marks
+ * an n_wp of 0 FUELGPU_POLY_BAD_INPUT and leaves the other rows alone, so fuelgpu_astar_batch_dev ->
+ * fuelgpu_poly_waypoints_batch_dev -> ... needs no host sync.  A MID tour (1.5 <= length <= 5.0) is written too: the
+ * reference calls kinodynamicReplan there instead, which this library does not replace, so the caller decides.
+ * Scratch: one map-owned device buffer, grown on demand: W warps search at once, W = min(B, 32 * SM count,
+ * max(1, 4 GiB / S)), with S = 80 * allocate_num + 16 * T + 24 bytes per warp (each array rounded up to 256 bytes), T the
+ * least power of two >= max(64, 2 * allocate_num), and 256 bytes more; FUELGPU_ENOMEM if it cannot be allocated.  Runs on the map's main stream;
+ * not timed in fuelgpu_map_last_timing.  The host entry returns FUELGPU_EINVAL and writes nothing on a non-finite start
+ * or goal or a bad parameter; the _dev entry checks the parameters alone and marks a row with a non-finite start or goal
+ * FUELGPU_ASTAR_BAD_INPUT, leaving the other rows unaffected. */
+#define FUELGPU_ASTAR_REACH_END 1 /* Astar::REACH_END */
+#define FUELGPU_ASTAR_NO_PATH 2   /* Astar::NO_PATH */
+/* FuelPathInfo.reason */
+#define FUELGPU_ASTAR_FOUND 0
+#define FUELGPU_ASTAR_OPEN_EMPTY 1 /* the open set ran empty (:144-148) */
+#define FUELGPU_ASTAR_POOL 2       /* use_node_num_ == allocate_num_ right after an allocation (:127-130) */
+#define FUELGPU_ASTAR_ITER_CAP 3   /* loop iteration max_iter + 1 (the reference's time cut, :75-79) */
+#define FUELGPU_ASTAR_HEAP_FULL 4  /* more than 2 * allocate_num open-set entries (device only) */
+#define FUELGPU_ASTAR_BAD_INPUT 5  /* _dev only: a non-finite start or goal */
+/* FuelPathInfo.branch (fast_exploration_manager.cpp:243-275) */
+#define FUELGPU_ASTAR_NONE 0
+#define FUELGPU_ASTAR_CLOSE 1 /* length < 1.5: the whole tour, next_goal = goal */
+#define FUELGPU_ASTAR_MID 2   /* otherwise: the reference runs kinodynamicReplan; the whole tour, next_goal = goal */
+#define FUELGPU_ASTAR_FAR 3   /* length > 5.0: the tour truncated past 5 m, next_goal = its last point */
+/* FuelPathInfo.tour_status */
+#define FUELGPU_ASTAR_TOO_LONG 1   /* more than FUELGPU_MAX_WAYPTS or w_max points */
+#define FUELGPU_ASTAR_DEGENERATE 2 /* fewer than 3 points */
+typedef struct {
+  double resolution;    /* astar/resolution_astar */
+  double lambda_heu;    /* astar/lambda_heu */
+  int32_t allocate_num; /* astar/allocate_num: the node pool */
+  int32_t max_iter;     /* stands for astar/max_search_time: loop iterations instead of seconds */
+} FuelAstarParams;
+typedef struct {
+  int32_t status;       /* FUELGPU_ASTAR_REACH_END or FUELGPU_ASTAR_NO_PATH */
+  int32_t reason;       /* FUELGPU_ASTAR_FOUND ... FUELGPU_ASTAR_BAD_INPUT */
+  int32_t iter_num, use_node_num, n_path; /* iter_num_, use_node_num_, getPath().size() */
+  int32_t n_wp;         /* points of the tour (0 without a path) */
+  int32_t branch;       /* FUELGPU_ASTAR_NONE / CLOSE / MID / FAR */
+  int32_t tour_status;  /* 0, FUELGPU_ASTAR_TOO_LONG, FUELGPU_ASTAR_DEGENERATE */
+  double early_terminate_cost; /* getEarlyTerminateCost() after FUELGPU_ASTAR_ITER_CAP, else 0 */
+  double length;               /* pathLength of the shortened path (0 without a path) */
+  double next_goal[3];         /* ed_->next_goal_ (0 without a path) */
+} FuelPathInfo;
+FUELGPU_API int fuelgpu_astar_batch(FuelMap* map, int32_t B, const double* start, const double* goal,
+                                    const FuelAstarParams* params, FuelPathInfo* info, int32_t path_max, double* path,
+                                    int32_t w_max, int32_t* n_wp, double* waypts);
+FUELGPU_API int fuelgpu_astar_batch_dev(FuelMap* map, int32_t B, const void* start_dev, const void* goal_dev,
+                                        const FuelAstarParams* params, void* info_dev, int32_t path_max, void* path_dev,
+                                        int32_t w_max, void* n_wp_dev, void* waypts_dev);
+
 /* ---- multi-GPU: the z-sharded ESDF update (BASELINE config 4; SURVEY 8e row 1) ---------------------------
  * Multi-GPU form of SDFMap::updateESDF3d (plan_env/src/sdf_map.cpp:152-241) over the whole map.  One process
  * (or thread) per GPU; rank r owns planes [r*nz/G, (r+1)*nz/G) of every (x,y) column, z fastest like the

@@ -302,6 +302,69 @@ private:
   double resolution_inv_ = 10.0;
 };
 
+// ---- Astar (path_searching/include/path_searching/astar2.h) over fuelgpu_astar_batch -----------------------
+// One search per call on the device of the environment's map.  init() takes the astar/* parameters as a struct;
+// max_search_time_ is an iteration cap here (max_iter): NO_PATH at loop iteration max_iter + 1.
+struct AstarParam {
+  double resolution_astar = 0.1, lambda_heu = 10000.0;
+  int allocate_num = 100000, max_iter = 100000;
+};
+class Astar {
+public:
+  enum { REACH_END = 1, NO_PATH = 2 };
+  void init(const AstarParam& p, const EDTEnvironment::Ptr& env) {
+    resolution_ = p.resolution_astar;
+    lambda_heu_ = p.lambda_heu;
+    allocate_num_ = p.allocate_num;
+    max_iter = p.max_iter;
+    edt_env_ = env;
+  }
+  void setResolution(const double& res) { resolution_ = res; }
+  void reset() {
+    path_nodes_.clear();
+    use_node_num_ = iter_num_ = 0;
+  }
+  int search(const Vector3d& start_pt, const Vector3d& end_pt) {
+    FuelMap* h = edt_env_->sdf_map_->gpu();
+    const FuelAstarParams ap{ resolution_, lambda_heu_, allocate_num_, max_iter };
+    const double s[3] = { start_pt(0), start_pt(1), start_pt(2) }, e[3] = { end_pt(0), end_pt(1), end_pt(2) };
+    FuelPathInfo info;
+    int32_t n_wp = 0;
+    std::vector<double> path(3 * ((size_t)allocate_num_ + 1));  // getPath() has at most allocate_num + 1 points
+    double wp[3 * FUELGPU_MAX_WAYPTS];
+    fuelgpu_check(fuelgpu_astar_batch(h, 1, s, e, &ap, &info, allocate_num_ + 1, path.data(), FUELGPU_MAX_WAYPTS, &n_wp,
+                                      wp),
+                  h);
+    use_node_num_ = info.use_node_num;
+    iter_num_ = info.iter_num;
+    if (info.reason == FUELGPU_ASTAR_ITER_CAP) early_terminate_cost_ = info.early_terminate_cost;
+    path_nodes_.clear();
+    for (int i = 0; i < info.n_path; ++i) path_nodes_.push_back(Vector3d(path[3 * i], path[3 * i + 1], path[3 * i + 2]));
+    return info.status;
+  }
+  std::vector<Vector3d> getPath() { return path_nodes_; }
+  static double pathLength(const std::vector<Vector3d>& path) {  // astar2.cpp:169-175
+    double length = 0.0;
+    for (size_t i = 0; i + 1 < path.size(); ++i) {
+      const double dx = path[i + 1](0) - path[i](0), dy = path[i + 1](1) - path[i](1), dz = path[i + 1](2) - path[i](2);
+      length += std::sqrt((dx * dx + dy * dy) + dz * dz);
+    }
+    return length;
+  }
+  double getEarlyTerminateCost() { return early_terminate_cost_; }
+  int use_node_num() const { return use_node_num_; }
+  int iter_num() const { return iter_num_; }
+
+  double lambda_heu_ = 10000.0;
+  int max_iter = 100000;  // stands for max_search_time_
+
+private:
+  EDTEnvironment::Ptr edt_env_;
+  std::vector<Vector3d> path_nodes_;
+  double resolution_ = 0.1, early_terminate_cost_ = 0.0;
+  int allocate_num_ = 100000, use_node_num_ = 0, iter_num_ = 0;
+};
+
 // ---- FrontierFinder (frontier_finder.h:25-131) ---------------------------------------------------
 struct Viewpoint {  // frontier_finder.h:25-31
   Vector3d pos_;
