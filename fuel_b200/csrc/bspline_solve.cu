@@ -40,8 +40,7 @@ __device__ __forceinline__ double dot3(const V3& a, const V3& b) {
 
 __global__ void __launch_bounds__(WPB * 32, 3) optimize_warp_kernel(
     Geom g, const float* __restrict__ dist, FuelOptParams p, const FuelTrajConst* __restrict__ tc, int n,
-    int mask, int B, FuelSolveParams sp, double* __restrict__ x, double* __restrict__ fbest,
-    int* __restrict__ neval_out) {
+    int mask, int B, FuelSolveParams sp, double* __restrict__ x, int* __restrict__ neval_out) {
   extern __shared__ double hist[];  // [WPB][2][m][32][3]
   const int lane = threadIdx.x & 31;
   const int w = threadIdx.x >> 5;
@@ -53,7 +52,7 @@ __global__ void __launch_bounds__(WPB * 32, 3) optimize_warp_kernel(
   double* S = hist + (size_t)w * 2 * m * 96;
   double* Y = S + (size_t)m * 96;
   double* xb = x + (int64_t)b * nvar;
-  TrajFast t;  // the faithful evaluator's constants are loaded after the loop, for the final evaluation only
+  TrajFast t;
   load_traj_fast(tc + b, t);
   const double knot_span = tc[b].knot_span;
 
@@ -89,14 +88,13 @@ __global__ void __launch_bounds__(WPB * 32, 3) optimize_warp_kernel(
     go.v[1] = is_pt ? gr[1] : 0.0;
     go.v[2] = is_pt ? gr[2] : 0.0;
   };
-  auto store_best = [&](const V3& xx, double fv) {
+  auto store_best = [&](const V3& xx) {
     if (is_pt) {
       xb[3 * lane] = xx.v[0];
       xb[3 * lane + 1] = xx.v[1];
       xb[3 * lane + 2] = xx.v[2];
     }
     if (is_dt) xb[nvar - 1] = xx.v[0];
-    if (lane == 0) fbest[b] = fv;
   };
 
   double F;
@@ -104,7 +102,7 @@ __global__ void __launch_bounds__(WPB * 32, 3) optimize_warp_kernel(
   evaluate(X, F, G);
   int neval = 1;
   double best = F;
-  store_best(X, F);
+  store_best(X);
   // a NaN/inf start cannot be improved on by comparison; treat as +inf
   if (!(best == best)) best = 1.7976931348623157e308;
 
@@ -201,7 +199,7 @@ __global__ void __launch_bounds__(WPB * 32, 3) optimize_warp_kernel(
       ++neval;
       if (FN < best) {  // costFunction :698-704
         best = FN;
-        store_best(XN, FN);
+        store_best(XN);
       }
       double dec = step * gd;  // = G.(XN - X) as long as no component hit a bound
       if (__any_sync(0xffffffffu, clipped)) {
@@ -251,21 +249,6 @@ __global__ void __launch_bounds__(WPB * 32, 3) optimize_warp_kernel(
     F = FN;
     G = GN;
     if (!exact && __all_sync(0xffffffffu, small)) break;  // xtol_rel, :173
-  }
-  // min_cost_ is reported from the full-precision evaluator (fp64 trilinear, per-term reductions) at
-  // the returned best_variable_, so it equals what combineCost gives for that x.
-  {
-    __syncwarp();
-    V3 XB;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) XB.v[k] = is_pt ? xb[3 * lane + k] : 0.0;
-    if (is_dt) XB.v[0] = xb[nvar - 1];
-    TrajRegs tr;
-    load_traj(tc + b, tr);
-    const double dtv = opt_time ? __shfl_sync(0xffffffffu, XB.v[0], n) : tr.knot_span;
-    double fo, gr[3], gdt;
-    eval_warp(g, dist, p, tr, tc + b, n, mask, XB.v, dtv, lane, fo, gr, gdt);
-    if (lane == 0) fbest[b] = fo;
   }
   if (lane == 0) neval_out[b] = neval;
 }
@@ -342,8 +325,7 @@ __device__ __forceinline__ void gram_row(const float* __restrict__ r, float (&o)
 template <int M>  // history length, compile time: every recursion loop has static bounds (5*M + 1 <= 32 values per batch)
 __global__ void __launch_bounds__(SOLVER_WPB * 32, SOLVER_SM_WARPS / SOLVER_WPB) optimize_gram_kernel(
     Geom g, const float* __restrict__ dist, FuelOptParams p, const FuelTrajConst* __restrict__ tc, int n,
-    int mask, int B, FuelSolveParams sp, double* __restrict__ x, double* __restrict__ fbest,
-    int* __restrict__ neval_out) {
+    int mask, int B, FuelSolveParams sp, double* __restrict__ x, int* __restrict__ neval_out) {
   static_assert(5 * M + 1 <= 32, "the batched reduction holds 32 values");
   static_assert(M <= GROW && 2 * (M - 1) * (M - 1) + (M - 1) <= 64, "Gram rows hold GROW values; the age shift moves <= 2 per lane");
   constexpr int MAXM = M;  // (shadows the file-level bound: Gram arrays are M wide here)
@@ -378,7 +360,7 @@ __global__ void __launch_bounds__(SOLVER_WPB * 32, SOLVER_SM_WARPS / SOLVER_WPB)
   // ages >= cnt are masked in the recursion; zeros keep them finite
   for (int i = lane; i < 2 * M * GROW + 3 * GROW; i += 32) SYa[i] = 0.f;
   double* xb = x + (int64_t)b * nvar;
-  TrajFast t;  // the faithful evaluator's constants are loaded after the loop, for the final evaluation only
+  TrajFast t;
   load_traj_fast(tc + b, t);
   const double knot_span = tc[b].knot_span;
 
@@ -416,14 +398,13 @@ __global__ void __launch_bounds__(SOLVER_WPB * 32, SOLVER_SM_WARPS / SOLVER_WPB)
     go.v[2] = is_pt ? gr[2] : 0.0;
     PROF_ADD(0, t_eval);
   };
-  auto store_best = [&](const V3& xx, double fv) {
+  auto store_best = [&](const V3& xx) {
     if (is_pt) {
       xb[3 * lane] = xx.v[0];
       xb[3 * lane + 1] = xx.v[1];
       xb[3 * lane + 2] = xx.v[2];
     }
     if (is_dt) xb[nvar - 1] = xx.v[0];
-    if (lane == 0) fbest[b] = fv;
   };
   auto project = [&](const V3& xx, const V3& gg, V3& pg, bool actv[3]) {
 #pragma unroll
@@ -439,7 +420,7 @@ __global__ void __launch_bounds__(SOLVER_WPB * 32, SOLVER_SM_WARPS / SOLVER_WPB)
   evaluate(X, F, G);
   int neval = 1;
   double best = F;
-  store_best(X, F);
+  store_best(X);
   if (!(best == best)) best = 1.7976931348623157e308;
 
   const bool exact = (sp.flags & FUELGPU_SOLVE_EXACT_EVALS) != 0;
@@ -548,7 +529,7 @@ __global__ void __launch_bounds__(SOLVER_WPB * 32, SOLVER_SM_WARPS / SOLVER_WPB)
       ++neval;
       if (FN < best) {  // costFunction :698-704
         best = FN;
-        store_best(XN, FN);
+        store_best(XN);
       }
       double dec = step * (double)gd;
       if (__any_sync(0xffffffffu, clipped)) {
@@ -683,19 +664,6 @@ __global__ void __launch_bounds__(SOLVER_WPB * 32, SOLVER_SM_WARPS / SOLVER_WPB)
     PROF_ADD(2, t_red);
     if (!exact && __all_sync(0xffffffffu, small)) break;  // xtol_rel, :173
   }
-  {
-    __syncwarp();
-    V3 XB;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) XB.v[k] = is_pt ? xb[3 * lane + k] : 0.0;
-    if (is_dt) XB.v[0] = xb[nvar - 1];
-    TrajRegs tr;
-    load_traj(tc + b, tr);
-    const double dtv = opt_time ? __shfl_sync(0xffffffffu, XB.v[0], n) : tr.knot_span;
-    double fo, gr[3], gdt;
-    eval_warp(g, dist, p, tr, tc + b, n, mask, XB.v, dtv, lane, fo, gr, gdt);
-    if (lane == 0) fbest[b] = fo;
-  }
   if (lane == 0) neval_out[b] = neval;
 #ifdef FUEL_PROF
   if (lane == 0) {
@@ -709,35 +677,54 @@ __global__ void __launch_bounds__(SOLVER_WPB * 32, SOLVER_SM_WARPS / SOLVER_WPB)
 #endif
 }
 
+int ensure_bs_grad(FuelMap* m, size_t bytes) {  // freed with the map (fuelgpu_map_destroy)
+  if (bytes <= m->bs_grad_bytes) return 0;
+  if (m->bs_grad) cudaFree(m->bs_grad);
+  m->bs_grad = nullptr;
+  m->bs_grad_bytes = 0;
+  FUEL_CUDA(m, cudaMalloc(&m->bs_grad, bytes));
+  m->bs_grad_bytes = bytes;
+  return 0;
+}
+
 }  // namespace
 
+// The solver kernels write best_variable_ and the evaluation count; min_cost_ at the returned x then comes from the
+// faithful evaluator (bspline.cu, compiled without FMA contraction) on the same stream, so that f_best is exactly what
+// fuelgpu_bspline_cost_batch returns for that x at every n_pts.  (An evaluation inlined in this file would be contracted.)
 int bspline_optimize_batch_dev_impl(FuelMap* m, int B, int n_pts, int mask, const FuelOptParams* p,
                                     const FuelTrajConst* tc_dev, const FuelSolveParams* sp,
                                     double* x_dev, double* fbest_dev, int32_t* neval_dev) {
   if (B <= 0) return 0;
-  const int need = n_pts + ((mask & FUELGPU_MINTIME) ? 1 : 0);
-  if (need > 32)  // two control points per lane (bspline_solve_long.cu)
-    return bspline_optimize_long_impl(m, B, n_pts, mask, p, tc_dev, sp, x_dev, fbest_dev, neval_dev);
+  const int nvar = (mask & FUELGPU_MINTIME) ? 3 * n_pts + 1 : 3 * n_pts;
+  int rc = ensure_bs_grad(m, sizeof(double) * (size_t)B * nvar);
+  if (rc) return rc;
   static int use_vec = -1;  // FUELGPU_SOLVER=vec selects the vector-space two-loop recursion (A/B, debugging)
   if (use_vec < 0) {
     const char* e = getenv("FUELGPU_SOLVER");
     use_vec = (e && !strcmp(e, "vec")) ? 1 : 0;
   }
-  if (use_vec || sp->lbfgs_m != 6) {  // the coefficient-space kernel is instantiated for the default history length
+  if (n_pts + ((mask & FUELGPU_MINTIME) ? 1 : 0) > 32) {  // two control points per lane (bspline_solve_long.cu)
+    rc = bspline_optimize_long_impl(m, B, n_pts, mask, p, tc_dev, sp, x_dev, neval_dev);
+    if (rc) return rc;
+  } else if (use_vec || sp->lbfgs_m != 6) {  // the coefficient-space kernel is instantiated for the default history length
     const size_t smem = (size_t)WPB * 2 * sp->lbfgs_m * 96 * sizeof(double);
     FUEL_CUDA(m, cudaFuncSetAttribute(optimize_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     optimize_warp_kernel<<<(B + WPB - 1) / WPB, WPB * 32, smem, m->stream>>>(m->g, m->dist, *p, tc_dev, n_pts, mask, B, *sp,
-                                                                        x_dev, fbest_dev, neval_dev);
+                                                                        x_dev, neval_dev);
+    FUEL_LAUNCHES(m, 1);
+    FUEL_CUDA(m, cudaGetLastError());
   } else {
     constexpr int GM = 6;
     const size_t smem = (size_t)SOLVER_WPB * SOLVER_FLOATS(GM) * sizeof(float);
     FUEL_CUDA(m, cudaFuncSetAttribute(optimize_gram_kernel<GM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     optimize_gram_kernel<GM><<<(B + SOLVER_WPB - 1) / SOLVER_WPB, SOLVER_WPB * 32, smem, m->stream>>>(m->g, m->dist, *p, tc_dev, n_pts, mask, B, *sp,
-                                                                            x_dev, fbest_dev, neval_dev);
+                                                                            x_dev, neval_dev);
+    FUEL_LAUNCHES(m, 1);
+    FUEL_CUDA(m, cudaGetLastError());
   }
-  FUEL_LAUNCHES(m, 1);
-  FUEL_CUDA(m, cudaGetLastError());
-  return 0;
+  return bspline_cost_batch_dev_impl(m, B, n_pts, mask & ~FUELGPU_COST_FAST_EVAL, p, tc_dev, x_dev, fbest_dev,
+                                     (double*)m->bs_grad);
 }
 
 #ifdef FUEL_PROF

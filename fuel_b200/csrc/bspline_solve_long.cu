@@ -296,33 +296,18 @@ __global__ void __launch_bounds__(LONG_WPB * 32) optimize_long_kernel(
   if (lane == 0) neval_out[b] = neval;
 }
 
-int ensure_bs_grad(FuelMap* m, size_t bytes) {  // freed with the map (fuelgpu_map_destroy)
-  if (bytes <= m->bs_grad_bytes) return 0;
-  if (m->bs_grad) cudaFree(m->bs_grad);
-  m->bs_grad = nullptr;
-  m->bs_grad_bytes = 0;
-  FUEL_CUDA(m, cudaMalloc(&m->bs_grad, bytes));
-  m->bs_grad_bytes = bytes;
-  return 0;
-}
-
 }  // namespace
 
-// n_pts + dt > 32 lanes: the solver above, then min_cost_ at the returned best_variable_ from the faithful evaluator
-// (bspline.cu, cost_batch_thread_kernel for these sizes) on the same stream, so that f_best is exactly what
-// fuelgpu_bspline_cost_batch returns for that x.
+// n_pts + dt > 32 lanes: the solver above (bspline_optimize_batch_dev_impl then takes min_cost_ at the returned x from
+// the faithful evaluator)
 int bspline_optimize_long_impl(FuelMap* m, int B, int n_pts, int mask, const FuelOptParams* p,
                                const FuelTrajConst* tc_dev, const FuelSolveParams* sp, double* x_dev,
-                               double* fbest_dev, int32_t* neval_dev) {
-  const int nvar = (mask & FUELGPU_MINTIME) ? 3 * n_pts + 1 : 3 * n_pts;
-  int rc = ensure_bs_grad(m, sizeof(double) * (size_t)B * nvar);
-  if (rc) return rc;
+                               int32_t* neval_dev) {
   const size_t smem = (size_t)LONG_WPB * LONG_SMEM_BYTES(sp->lbfgs_m);
   FUEL_CUDA(m, cudaFuncSetAttribute(optimize_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   optimize_long_kernel<<<(B + LONG_WPB - 1) / LONG_WPB, LONG_WPB * 32, smem, m->stream>>>(m->g, m->dist, *p, tc_dev, n_pts,
                                                                                      mask, B, *sp, x_dev, neval_dev);
   FUEL_LAUNCHES(m, 1);
   FUEL_CUDA(m, cudaGetLastError());
-  return bspline_cost_batch_dev_impl(m, B, n_pts, mask & ~FUELGPU_COST_FAST_EVAL, p, tc_dev, x_dev, fbest_dev,
-                                     (double*)m->bs_grad);
+  return 0;
 }

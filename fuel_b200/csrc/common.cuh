@@ -173,7 +173,7 @@ int bspline_optimize_batch_dev_impl(FuelMap* m, int B, int n_pts, int mask, cons
                                     double* x_dev, double* fbest_dev, int32_t* neval_dev);
 int bspline_optimize_long_impl(FuelMap* m, int B, int n_pts, int mask, const FuelOptParams* p,
                                const FuelTrajConst* tc_dev, const FuelSolveParams* sp, double* x_dev,
-                               double* fbest_dev, int32_t* neval_dev);
+                               int32_t* neval_dev);
 // traj_check.cu: NonUniformBspline checks / checkTrajCollision / selectBestTraj, and evaluateDeBoorT
 int traj_check_impl(FuelMap* m, int B, int n_pts, int nvar, const double* x_dev, const double* dt_dev,
                     const FuelTrajCheckParams* p, FuelTrajReport* rep_dev, int32_t* best_dev);

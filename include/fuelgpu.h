@@ -357,8 +357,9 @@ FUELGPU_API int fuelgpu_bspline_cost_batch_dev(FuelMap* map, int32_t B, int32_t 
  * L-BFGS run per trajectory inside one persistent kernel; iterate-level parity with NLopt
  * is unpinned (SURVEY 8c), the CPU twin is oracle/orc_optimize_batch.
  * x [B][nvar] in/out (best_variable_), f_best [B], n_eval [B].  n_pts <= 64: up to 32 lanes (n_pts + dt) one
- * control point per lane, above that two per lane (and f_best is then exactly what fuelgpu_bspline_cost_batch returns
- * for the returned x). */
+ * control point per lane, above that two per lane.  At every n_pts, f_best is exactly (bit for bit) what
+ * fuelgpu_bspline_cost_batch returns for the returned x: the faithful evaluator runs on it after the solver, on the
+ * same stream. */
 typedef struct {
   int32_t max_eval; /* max_iteration_num_[id]  (algorithm.xml:184-187) */
   int32_t lbfgs_m;  /* history pairs, <= 8                              */
