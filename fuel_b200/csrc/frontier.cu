@@ -1241,6 +1241,9 @@ __global__ void init_meta_kernel(ClusterMeta* meta, ClusterStat* st, LevelCtl ct
 constexpr int SMALL_CTAS = 8;      // one thread-block cluster (portable maximum)
 constexpr int SMALL_CAP = 32768;   // candidate cells
 constexpr int SMALL_CCAP = 8192;   // clusters (incl. split products)
+// the speculative prefix of the small path's results that comes back with the counters in one copy: a search with more
+// kept cells or clusters fetches the rest with a second, exact-size download
+constexpr int RES_K0 = 12288, RES_C0 = 256;
 
 
 // Small path: the kept/root marks of 32 consecutive cells are one ballot, so the rank scan runs over ceil(n/32) <= 1024
@@ -1322,6 +1325,14 @@ struct SmallBufs {
   ClusterMeta* meta;
   ClusterStat* stat;
   int* counters;  // [0] n_cand (in) [1] R [2] K [3] n_new [4] status [5] C
+  // the result block the host fetches with ONE copy: the eight counters, then the first r_C clusters and r_K kept
+  // cells of meta / stat / k_addr / k_cl / k_leaf / k_cent, laid out as the pinned buffer (result_layout)
+  int* r_counters;
+  ClusterMeta* r_meta;
+  ClusterStat* r_stat;
+  int *r_addr, *r_cl, *r_leaf;
+  float* r_cent;
+  int r_K, r_C;
 };
 
 __global__ void __cluster_dims__(SMALL_CTAS, 1, 1) __launch_bounds__(1024) cluster_small_kernel(Geom g, FParams fp, int8_t* __restrict__ flag,
@@ -1342,7 +1353,11 @@ __global__ void __cluster_dims__(SMALL_CTAS, 1, 1) __launch_bounds__(1024) clust
 #endif
   STAMP();
   if (n > SMALL_CAP) {
-    if (tid == 0) b.counters[4] = 1;
+    if (tid == 0) {
+      b.counters[4] = 1;
+      b.r_counters[0] = n;
+      b.r_counters[4] = 1;
+    }
     return;  // uniform over the whole cluster
   }
 #define FOR_ITEMS(i, N) for (int i = tid; i - tid < (N); i += NT)  // uniform trip count per warp
@@ -1417,9 +1432,33 @@ __global__ void __cluster_dims__(SMALL_CTAS, 1, 1) __launch_bounds__(1024) clust
     }
   }
   FOR_ITEMS(i, n) reset_cellidx_item(b.cell_addr, cellidx, n, i);
+  // the prefix of the results the host reads goes into the result block (every value is final since the last
+  // cluster.sync(), whichever CTA wrote it)
+  if (status == 0 && R > 0 && K > 0) {
+    const int kp = min(K, b.r_K), cp = min(C, b.r_C);
+    FOR_ITEMS(k, kp) {
+      if (k < kp) {
+        b.r_addr[k] = b.k_addr[k];
+        b.r_cl[k] = b.k_cl[k];
+        b.r_leaf[k] = b.k_leaf[k];
+        b.r_cent[3 * k] = b.k_cent[3 * k];
+        b.r_cent[3 * k + 1] = b.k_cent[3 * k + 1];
+        b.r_cent[3 * k + 2] = b.k_cent[3 * k + 2];
+      }
+    }
+    FOR_ITEMS(c, cp) {
+      if (c < cp) {
+        b.r_meta[c] = b.meta[c];
+        b.r_stat[c] = b.stat[c];
+      }
+    }
+  }
   if (tid == 0) {
     b.counters[4] = status;
     b.counters[5] = C;
+    const int out[8] = { n, R, K, b.counters[3], status, C, b.counters[6], b.counters[7] };
+#pragma unroll
+    for (int j = 0; j < 8; ++j) b.r_counters[j] = out[j];
   }
 #undef FOR_ITEMS
 }
@@ -1510,6 +1549,7 @@ struct FrontierState {
   DevBuf<float> k_cent;
   DevBuf<ClusterStat> stat;
   DevBuf<ClusterMeta> meta;
+  DevBuf<char> res;  // the small path's result block (SmallBufs::r_*), fetched with one copy
   bool small_ready = false;
   // a search that has been enqueued (begin) but not yet collected (end)
   bool pend_active = false, pend_empty = true;
@@ -1579,7 +1619,7 @@ void frontier_state_destroy(FuelMap* m) {
   f->cell_addr.release(); f->parent.release(); f->claim.release(); f->csize.release();
   f->seed.release(); f->is_root.release(); f->is_kept.release(); f->root_rank.release();
   f->kept_off.release(); f->cell_cls.release(); f->k_addr.release(); f->k_cl.release();
-  f->k_leaf.release(); f->k_cent.release(); f->stat.release(); f->meta.release();
+  f->k_leaf.release(); f->k_cent.release(); f->stat.release(); f->meta.release(); f->res.release();
   delete f;
   m->fs = nullptr;
 }
@@ -1673,23 +1713,51 @@ static int ensure_pin(FuelMap* m, size_t bytes) {
   return 0;
 }
 
+// byte offsets of the arrays of K cells / C clusters in a result buffer (16-byte aligned pieces)
+struct ResultLayout {
+  size_t meta, stat, addr, cl, leaf, cent, bytes;
+};
+static ResultLayout result_layout(int K, int C) {
+  ResultLayout l;
+  size_t p = 0;
+  auto put = [&](size_t bytes) {
+    const size_t o = p;
+    p += (bytes + 15) & ~(size_t)15;
+    return o;
+  };
+  l.meta = put(sizeof(ClusterMeta) * C);
+  l.stat = put(sizeof(ClusterStat) * C);
+  l.addr = put(sizeof(int) * K);
+  l.cl = put(sizeof(int) * K);
+  l.leaf = put(sizeof(int) * K);
+  l.cent = put(sizeof(float) * 3 * K);
+  l.bytes = p;
+  return l;
+}
+static void result_view(const ResultLayout& l, const char* base, HostView* v) {
+  v->meta = (const ClusterMeta*)(base + l.meta);
+  v->stat = (const ClusterStat*)(base + l.stat);
+  v->addr = (const int*)(base + l.addr);
+  v->cl = (const int*)(base + l.cl);
+  v->leaf = (const int*)(base + l.leaf);
+  v->cent = (const float*)(base + l.cent);
+}
+
 // enqueue the D2H of K cells / C clusters into the pinned buffer at `base` (no sync)
 static int enqueue_download(FuelMap* m, int K, int C, char* base, HostView* v) {
   FrontierState* f = m->fs;
   cudaStream_t s = m->fs->stream;
-  char* p = base;
-  auto put = [&](const void* src, size_t bytes) -> char* {
-    char* dst = p;
-    p += (bytes + 15) & ~(size_t)15;
-    if (bytes) cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s);
-    return dst;
+  const ResultLayout l = result_layout(K, C);
+  result_view(l, base, v);
+  auto get = [&](const void* dst, const void* src, size_t bytes) {
+    if (bytes) cudaMemcpyAsync((void*)dst, src, bytes, cudaMemcpyDeviceToHost, s);
   };
-  v->meta = (const ClusterMeta*)put(f->meta.p, sizeof(ClusterMeta) * C);
-  v->stat = (const ClusterStat*)put(f->stat.p, sizeof(ClusterStat) * C);
-  v->addr = (const int*)put(f->k_addr.p, sizeof(int) * K);
-  v->cl = (const int*)put(f->k_cl.p, sizeof(int) * K);
-  v->leaf = (const int*)put(f->k_leaf.p, sizeof(int) * K);
-  v->cent = (const float*)put(f->k_cent.p, sizeof(float) * 3 * K);
+  get(v->meta, f->meta.p, sizeof(ClusterMeta) * C);
+  get(v->stat, f->stat.p, sizeof(ClusterStat) * C);
+  get(v->addr, f->k_addr.p, sizeof(int) * K);
+  get(v->cl, f->k_cl.p, sizeof(int) * K);
+  get(v->leaf, f->k_leaf.p, sizeof(int) * K);
+  get(v->cent, f->k_cent.p, sizeof(float) * 3 * K);
   FUEL_CUDA(m, cudaGetLastError());
   return 0;
 }
@@ -2009,6 +2077,10 @@ int frontier_search_begin_impl(FuelMap* m, const double umin[3], const double um
     ENSURE(f->kept_off, SMALL_CAP); ENSURE(f->k_addr, SMALL_CAP); ENSURE(f->k_cl, SMALL_CAP);
     ENSURE(f->k_leaf, SMALL_CAP); ENSURE(f->k_cent, (size_t)3 * SMALL_CAP);
     ENSURE(f->meta, SMALL_CCAP); ENSURE(f->stat, SMALL_CCAP);
+    // one host sync and ONE copy in the common case: the kernel writes the counters and a speculative prefix of the
+    // results (RES_K0 cells, RES_C0 clusters) into one block; a second download only if they did not fit
+    const ResultLayout rl = result_layout(RES_K0, RES_C0);
+    ENSURE(f->res, 64 + rl.bytes);
     sweep_compact(m, fp, pl, f->cellidx, SMALL_CAP, s);
     SmallBufs sb;
     sb.cell_addr = f->cell_addr.p; sb.parent = f->parent.p; sb.claim = f->claim.p; sb.csize = f->csize.p;
@@ -2016,18 +2088,21 @@ int frontier_search_begin_impl(FuelMap* m, const double umin[3], const double um
     sb.kept_off = f->kept_off.p; sb.cell_cls = f->cell_cls.p; sb.k_addr = f->k_addr.p; sb.k_cl = f->k_cl.p;
     sb.k_leaf = f->k_leaf.p; sb.k_cent = f->k_cent.p; sb.meta = f->meta.p; sb.stat = f->stat.p;
     sb.counters = f->d_counters;
+    {
+      char* rb = f->res.p + 64;
+      sb.r_counters = (int*)f->res.p;
+      sb.r_meta = (ClusterMeta*)(rb + rl.meta); sb.r_stat = (ClusterStat*)(rb + rl.stat);
+      sb.r_addr = (int*)(rb + rl.addr); sb.r_cl = (int*)(rb + rl.cl); sb.r_leaf = (int*)(rb + rl.leaf);
+      sb.r_cent = (float*)(rb + rl.cent);
+      sb.r_K = RES_K0;
+      sb.r_C = RES_C0;
+    }
     cluster_small_kernel<<<SMALL_CTAS, 1024, 0, s>>>(g, fp, m->flag, f->cellidx, sb);
     FUEL_LAUNCHES(m, 1);
-    // one host sync in the common case: the counters and a speculative prefix of the results
-    // (K0 cells, C0 clusters) are downloaded together; a second stage only if they did not fit
-    constexpr int K0 = 12288, C0 = 256;
-    int rc0 = ensure_pin(m, 64 + view_bytes(K0, C0));
+    int rc0 = ensure_pin(m, 64 + rl.bytes);
     if (rc0) return rc0;
-    int* cnt = (int*)f->h_pin;
-    FUEL_CUDA(m, cudaMemcpyAsync(cnt, f->d_counters, sizeof(int) * 8, cudaMemcpyDeviceToHost, s));
-    HostView& hv = f->pend_hv;
-    rc0 = enqueue_download(m, K0, C0, f->h_pin + 64, &hv);
-    if (rc0) return rc0;
+    FUEL_CUDA(m, cudaMemcpyAsync(f->h_pin, f->res.p, 64 + rl.bytes, cudaMemcpyDeviceToHost, s));
+    result_view(rl, f->h_pin + 64, &f->pend_hv);
     f->pend_fp = fp;
     f->pend_plan = pl;
     f->pend_active = true;
@@ -2053,8 +2128,7 @@ int frontier_search_end_impl(FuelMap* m, int32_t* n_clusters, int32_t* n_cells, 
   const SweepPlan pl = f->pend_plan;
   int n_cand = 0;
   {
-    constexpr int K0 = 12288, C0 = 256;
-    int* cnt = (int*)f->h_pin;
+    const int* cnt = (const int*)f->h_pin;
     HostView& hv = f->pend_hv;
     FUEL_CUDA(m, cudaStreamSynchronize(s));
     n_cand = cnt[0];
@@ -2062,7 +2136,7 @@ int frontier_search_end_impl(FuelMap* m, int32_t* n_clusters, int32_t* n_cells, 
     if (cnt[4] == 0) {
       const int R = cnt[1], K = cnt[2], C = cnt[5];
       if (R == 0 || K == 0) return 0;
-      if (K <= K0 && C <= C0) return frontier_build_csr(m, K, C, hv, n_clusters, n_cells, n_filtered);
+      if (K <= RES_K0 && C <= RES_C0) return frontier_build_csr(m, K, C, hv, n_clusters, n_cells, n_filtered);
       return frontier_marshal(m, K, C, n_clusters, n_cells, n_filtered);
     }
     // capacity exceeded (status 1: cells, 2: clusters): fall through to the multi-kernel path.

@@ -15,6 +15,11 @@ import numpy as np
 from ._lib import FuelFrontierParams, FuelViewParams, check, lib, ptr
 
 
+def _data(a):
+    """address of a numpy array's first element, as an int (ctypes passes it as void*)"""
+    return a.__array_interface__["data"][0]
+
+
 class Frontier:
     """frontier_finder.h:34-51"""
     __slots__ = ("cells_addr_", "filtered_cells_", "average_", "id_", "box_min_", "box_max_", "_map", "viewpoints_")
@@ -155,7 +160,7 @@ class FrontierFinder:
         umin = np.ascontiguousarray(update_min, dtype=np.float64)
         umax = np.ascontiguousarray(update_max, dtype=np.float64)
         p = self._params()
-        check(lib().fuelgpu_frontier_search_begin(h, ptr(umin), ptr(umax), C.byref(p)), h)
+        check(lib().fuelgpu_frontier_search_begin(h, _data(umin), _data(umax), C.byref(p)), h)
 
     def candidates(self, update_min, update_max, z_lo, z_hi):
         """The sweep of the planes [z_lo, z_hi] only (fuelgpu_frontier_candidates): this rank's candidate cells of a
@@ -195,17 +200,19 @@ class FrontierFinder:
     def _fetch(self, nc, ncell, nf):
         m = self._map
         h = m.handle
-        # arrays of this call; the Frontier objects hold views into them
+        # arrays of this call; the Frontier objects hold views into them.  This runs once per search, on the replan's
+        # critical path: the pointers are taken as plain integers (ndarray.ctypes costs several microseconds each)
         offs = np.empty(nc + 1, dtype=np.int32)
         addr = np.empty(ncell, dtype=np.int32)
         foffs = np.empty(nc + 1, dtype=np.int32)
         filt = np.empty((nf, 3), dtype=np.float64)
         stats = np.empty((3, nc, 3), dtype=np.float64)
-        avg, bmin, bmax = stats[0], stats[1], stats[2]
-        check(lib().fuelgpu_frontier_fetch(h, ptr(offs), ptr(addr), ptr(foffs), ptr(filt), ptr(avg), ptr(bmin),
-                                           ptr(bmax)), h)
+        s0 = _data(stats)
+        check(lib().fuelgpu_frontier_fetch(h, _data(offs), _data(addr), _data(foffs), _data(filt), s0, s0 + 24 * nc,
+                                           s0 + 48 * nc), h)
         o, fo = offs.tolist(), foffs.tolist()
-        return [Frontier(m, addr[o[i]:o[i + 1]], filt[fo[i]:fo[i + 1]], avg[i], bmin[i], bmax[i]) for i in range(nc)]
+        return [Frontier(m, addr[o[i]:o[i + 1]], filt[fo[i]:fo[i + 1]], a, lo, hi)
+                for i, (a, lo, hi) in enumerate(zip(stats[0], stats[1], stats[2]))]
 
     # ---- the step after the search (SURVEY 8f rank 4) -------------------------------------
     def sampleViewpointsRaw(self, ftrs):
