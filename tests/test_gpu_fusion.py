@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 
 from fuel_b200 import workloads as W
+from tests.esdf_exact import check_esdf
 from tests.helpers import orc_grid
 
 pytestmark = pytest.mark.gpu
@@ -101,11 +102,7 @@ def test_office_depth_frames_then_inflate_and_esdf(fuel, orc):
         assert np.array_equal(m.occupancy_buffer_inflate_, inf_o)
         m.updateESDF3d()
         got = m.download(lo, hi).copy()
-        sl = tuple(slice(lo[i], hi[i] + 1) for i in range(3))
-        r, q = ref[sl], got[sl]
-        fin = r < 1e150
-        assert np.array_equal(np.isinf(q), ~fin)
-        assert np.all(np.abs(q[fin] - r[fin]) <= 1e-4 * np.abs(r[fin]))
+        check_esdf(got, ref, g.res, box=(lo, hi))
     m.close()
 
 

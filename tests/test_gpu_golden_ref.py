@@ -1,7 +1,8 @@
 """The CUDA path (through the C ABI) against golden OUTPUT vectors of the reference's own code
 (tests/golden/ref_outputs.npz, written by tools/make_ref_golden.py from oracle/_ref = the reference's sdf_map.cpp,
 frontier_finder.cpp, bspline_optimizer.cpp ... compiled unmodified in the build container).  No oracle in between.
-Bars: ESDF <= 1e-4 relative with +inf where the reference holds its DBL_MAX sentinel; frontier clusters, cell sets,
+Bars: ESDF at the exact bar of tests/esdf_exact.py (the stored fp32 values still determine the squared voxel
+distance) with +inf where the reference holds its DBL_MAX sentinel; frontier clusters, cell sets,
 flags bit-exact, filtered cells to the last float32 bit (cells of a cluster in ascending address on the device, BFS
 order in the reference: compared as sorted sets, DESIGN.md "frontier cell order"); fused log-odds, local bounds, inflation bit-exact;
 combineCost cost and gradient <= 1e-4; viewpoint positions exact, yaw <= 1e-9 rad, visible counts equal."""
@@ -11,6 +12,7 @@ import numpy as np
 import pytest
 
 from fuel_b200 import workloads as W
+from tests.esdf_exact import check_esdf
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_outputs.npz")
@@ -43,11 +45,9 @@ def test_esdf_vs_reference(fuel, gold, name, opt, sgn):
     lo, hi = gold["esdf_lo"], gold["esdf_hi"]
     m.local_bound_min_, m.local_bound_max_ = lo, hi
     m.updateESDF3d()
-    got = m.download(lo, hi)[lo[0]:hi[0] + 1, lo[1]:hi[1] + 1, lo[2]:hi[2] + 1].astype(np.float64)
-    want = gold["esdf_" + name].astype(np.float64)
-    assert np.array_equal(np.isinf(got), np.isinf(want))
-    fin = np.isfinite(want)
-    assert np.all(np.abs(got[fin] - want[fin]) <= 1e-4 * np.abs(want[fin]) + 1e-7)
+    got = m.download(lo, hi)[lo[0]:hi[0] + 1, lo[1]:hi[1] + 1, lo[2]:hi[2] + 1]
+    want = gold["esdf_" + name]
+    check_esdf(got, want, float(gold["res"]), signed=sgn, ref_f32=True, label="golden " + name)
     m.close()
 
 
