@@ -59,36 +59,6 @@ __global__ void clear_flags_kernel(int8_t* flag, const int* __restrict__ addr, i
   if (i < n) flag[addr[i]] = 0;
 }
 
-int ensure_stage(FuelMap* m, size_t bytes) {
-  if (bytes <= m->stage_bytes) return 0;
-  if (m->stage) cudaFree(m->stage);
-  m->stage = nullptr;
-  m->stage_bytes = 0;
-  FUEL_CUDA(m, cudaMalloc(&m->stage, bytes));
-  m->stage_bytes = bytes;
-  return 0;
-}
-
-int ensure_bs(FuelMap* m, size_t bytes) {
-  if (bytes <= m->bs_bytes) return 0;
-  if (m->bs_buf) cudaFree(m->bs_buf);
-  m->bs_buf = nullptr;
-  m->bs_bytes = 0;
-  FUEL_CUDA(m, cudaMalloc(&m->bs_buf, bytes));
-  m->bs_bytes = bytes;
-  return 0;
-}
-
-static int ensure_bs_pin(FuelMap* m, size_t bytes) {
-  if (bytes <= m->bs_pin_bytes) return 0;
-  if (m->bs_pin) cudaFreeHost(m->bs_pin);
-  m->bs_pin = nullptr;
-  m->bs_pin_bytes = 0;
-  FUEL_CUDA(m, cudaMallocHost(&m->bs_pin, bytes + bytes / 4));
-  m->bs_pin_bytes = bytes + bytes / 4;
-  return 0;
-}
-
 int check_box(FuelMap* m, const int32_t bmin[3], const int32_t bmax[3], int lo[3], int hi[3]) {
   const int n[3] = { m->g.nx, m->g.ny, m->g.nz };
   for (int i = 0; i < 3; ++i) {
@@ -99,6 +69,64 @@ int check_box(FuelMap* m, const int32_t bmin[3], const int32_t bmax[3], int lo[3
   }
   return 0;
 }
+
+size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+// The host arrays of one host-facing batch call, staged in tc_buf in 256-byte aligned pieces.  in() and out() name
+// a device pointer and the host array it stands for; a null host array gives a null device pointer.  upload() lays
+// the arrays out and enqueues the copies of the inputs on m->stream; download() enqueues the copies of the outputs
+// and waits for them.
+class HostStaging {
+ public:
+  explicit HostStaging(FuelMap* m) : m_(m) {}
+  template <typename T>
+  HostStaging& in(T** dev, const T* host, size_t n) {
+    arrays_.push_back({ dev, nullptr, host, nullptr, sizeof(T) * n });
+    return *this;
+  }
+  template <typename T>
+  HostStaging& out(T** dev, T* host, size_t n) {
+    arrays_.push_back({ dev, nullptr, host, host, sizeof(T) * n });
+    return *this;
+  }
+  int upload() {
+    FuelMap* m = m_;
+    size_t total = 0;
+    for (const Array& a : arrays_)
+      if (a.host) total += align256(a.bytes);
+    int rc = m->tc_buf.ensure(m, total);
+    if (rc) return rc;
+    uint8_t* q = m->tc_buf.p;
+    for (Array& a : arrays_) {
+      if (a.host) {
+        a.dev = q;
+        q += align256(a.bytes);
+      }
+      memcpy(a.slot, &a.dev, sizeof(a.dev));  // *(T**)slot = dev, without type punning
+      if (a.host && !a.out && a.bytes)
+        FUEL_CUDA(m, cudaMemcpyAsync(a.dev, a.host, a.bytes, cudaMemcpyHostToDevice, m->stream));
+    }
+    return 0;
+  }
+  int download() {
+    FuelMap* m = m_;
+    for (const Array& a : arrays_)
+      if (a.out && a.bytes) FUEL_CUDA(m, cudaMemcpyAsync(a.out, a.dev, a.bytes, cudaMemcpyDeviceToHost, m->stream));
+    FUEL_CUDA(m, cudaStreamSynchronize(m->stream));
+    return 0;
+  }
+
+ private:
+  struct Array {
+    void* slot;       // the caller's T* that receives dev
+    void* dev;        // place in tc_buf, null for a null host array
+    const void* host;
+    void* out;        // the host array again for an output, null for an input
+    size_t bytes;
+  };
+  FuelMap* m_;
+  std::vector<Array> arrays_;
+};
 
 }  // namespace
 
@@ -148,7 +176,6 @@ int fuelgpu_map_create(const FuelGridDesc* grid, int device_id, FuelMap** out) {
 
   FuelMap* m = new (std::nothrow) FuelMap();
   if (!m) return fuel_fail(nullptr, FUELGPU_ENOMEM, "host allocation failed");
-  memset(m, 0, sizeof(*m));
   m->desc = *grid;
   m->dev = device_id;
   m->sm_count = prop.multiProcessorCount;
@@ -231,17 +258,22 @@ int fuelgpu_map_destroy(FuelMap* m) {
   if (m->own_stream) cudaStreamSynchronize(m->own_stream);
   frontier_state_destroy(m);
   fusion_state_destroy(m);
-  if (m->bs_pin) cudaFreeHost(m->bs_pin);
   if (m->esdf_aux) {
     cudaStreamSynchronize(m->esdf_aux);
     cudaStreamDestroy(m->esdf_aux);
   }
   for (int i = 0; i < 2; ++i)
     if (m->esdf_ev[i]) cudaEventDestroy(m->esdf_ev[i]);
-  void* ptrs[] = { m->occ,       m->dist,      m->dist_neg, m->flag,   m->esdf_rec,
-                   m->esdf_p[0], m->esdf_p[1], m->stage,    m->bs_buf, m->fr_scr, m->bs_grad, m->tc_buf, m->as_buf };
+  void* ptrs[] = { m->occ, m->dist, m->dist_neg, m->flag, m->esdf_rec, m->esdf_p[0], m->esdf_p[1] };
   for (void* p : ptrs)
     if (p) cudaFree(p);
+  m->stage.release();
+  m->bs_buf.release();
+  m->bs_pin.release();
+  m->bs_grad.release();
+  m->fr_scr.release();
+  m->tc_buf.release();
+  m->as_buf.release();
   for (int t = 0; t < T_COUNT; ++t) {
     if (m->ev0[t]) cudaEventDestroy(m->ev0[t]);
     if (m->ev1[t]) cudaEventDestroy(m->ev1[t]);
@@ -345,20 +377,20 @@ static int upload_occupancy_impl(FuelMap* m, const int8_t* inflate, const double
   const int64_t off = (int64_t)lo[0] * plane;
   const int64_t cnt = (int64_t)(hi[0] - lo[0] + 1) * plane;
   const size_t inf_bytes = ((size_t)cnt + 7) & ~(size_t)7;  // keeps the fp64 region 8-byte aligned
-  rc = ensure_stage(m, inf_bytes + (size_t)cnt * (logodds ? 8 : 1));
+  rc = m->stage.ensure(m, inf_bytes + (size_t)cnt * (logodds ? 8 : 1));
   if (rc) return rc;
   frontier_order_writer(m);
   tbegin(m, T_UPLOAD);
-  int8_t* d_inf = (int8_t*)m->stage;
+  int8_t* d_inf = (int8_t*)m->stage.p;
   FUEL_CUDA(m, cudaMemcpyAsync(d_inf, inflate + off, cnt, cudaMemcpyHostToDevice, m->stream));
   const unsigned nb = (unsigned)((cnt + 255) / 256);
   if (logodds) {
-    double* d_lo = (double*)((uint8_t*)m->stage + inf_bytes);
+    double* d_lo = (double*)(m->stage.p + inf_bytes);
     FUEL_CUDA(m, cudaMemcpyAsync(d_lo, logodds + off, cnt * 8, cudaMemcpyHostToDevice, m->stream));
     ingest_logodds_kernel<<<nb, 256, 0, m->stream>>>(d_inf, d_lo, m->occ + off, cnt, clamp_min_log - 1e-3,
                                                      min_occupancy_log);
   } else {
-    uint8_t* d_tri = (uint8_t*)m->stage + inf_bytes;
+    uint8_t* d_tri = m->stage.p + inf_bytes;
     FUEL_CUDA(m, cudaMemcpyAsync(d_tri, tristate + off, cnt, cudaMemcpyHostToDevice, m->stream));
     ingest_tri_kernel<<<nb, 256, 0, m->stream>>>(d_inf, d_tri, m->occ + off, cnt);
   }
@@ -459,10 +491,10 @@ int fuelgpu_map_get_logodds(FuelMap* m, double* logodds) {
 int fuelgpu_map_download_occupancy(FuelMap* m, int8_t* inflate, uint8_t* tristate) {
   if (!m || (!inflate && !tristate)) return fuel_fail(m, FUELGPU_EINVAL, "null argument");
   FUEL_CUDA(m, cudaSetDevice(m->dev));
-  int rc = ensure_stage(m, (size_t)m->nvox * 2);
+  int rc = m->stage.ensure(m, (size_t)m->nvox * 2);
   if (rc) return rc;
-  int8_t* d_inf = (int8_t*)m->stage;
-  uint8_t* d_tri = (uint8_t*)m->stage + m->nvox;
+  int8_t* d_inf = (int8_t*)m->stage.p;
+  uint8_t* d_tri = m->stage.p + m->nvox;
   split_occ_kernel<<<(unsigned)((m->nvox + 255) / 256), 256, 0, m->stream>>>(m->occ, d_inf, d_tri, m->nvox);
   FUEL_LAUNCHES(m, 1);
   FUEL_CUDA(m, cudaGetLastError());
@@ -501,13 +533,13 @@ int fuelgpu_esdf_download(FuelMap* m, const int32_t bmin[3], const int32_t bmax[
   if (out_f32) {
     FUEL_CUDA(m, cudaMemcpyAsync(out_f32 + off, m->dist + off, cnt * 4, cudaMemcpyDeviceToHost, m->stream));
   } else {
-    rc = ensure_stage(m, (size_t)cnt * 8);
+    rc = m->stage.ensure(m, (size_t)cnt * 8);
     if (rc) return rc;
     f32_to_f64_kernel<<<(unsigned)((cnt + 255) / 256), 256, 0, m->stream>>>(
-        m->dist + off, (double*)m->stage, cnt, m->g.res * sqrt(1.7976931348623157e308));
+        m->dist + off, (double*)m->stage.p, cnt, m->g.res * sqrt(1.7976931348623157e308));
     FUEL_LAUNCHES(m, 1);
     FUEL_CUDA(m, cudaGetLastError());
-    FUEL_CUDA(m, cudaMemcpyAsync(out_f64 + off, m->stage, cnt * 8, cudaMemcpyDeviceToHost, m->stream));
+    FUEL_CUDA(m, cudaMemcpyAsync(out_f64 + off, m->stage.p, cnt * 8, cudaMemcpyDeviceToHost, m->stream));
   }
   tend(m, T_DOWNLOAD);
   FUEL_CUDA(m, cudaStreamSynchronize(m->stream));
@@ -555,18 +587,14 @@ int fuelgpu_esdf_sample(FuelMap* m, int64_t n, const double* pos, double* dist, 
   if (!m || (n > 0 && (!pos || !dist || !grad))) return fuel_fail(m, FUELGPU_EINVAL, "null argument");
   if (n <= 0) return 0;
   FUEL_CUDA(m, cudaSetDevice(m->dev));
-  int rc = ensure_bs(m, (size_t)n * 7 * sizeof(double));
+  double *d_pos, *d_d, *d_g;
+  HostStaging st(m);
+  st.in(&d_pos, pos, 3 * (size_t)n).out(&d_d, dist, (size_t)n).out(&d_g, grad, 3 * (size_t)n);
+  int rc = st.upload();
   if (rc) return rc;
-  double* d_pos = (double*)m->bs_buf;
-  double* d_d = d_pos + 3 * n;
-  double* d_g = d_d + n;
-  FUEL_CUDA(m, cudaMemcpyAsync(d_pos, pos, sizeof(double) * 3 * n, cudaMemcpyHostToDevice, m->stream));
   rc = esdf_sample_impl(m, n, d_pos, d_d, d_g);
   if (rc) return rc;
-  FUEL_CUDA(m, cudaMemcpyAsync(dist, d_d, sizeof(double) * n, cudaMemcpyDeviceToHost, m->stream));
-  FUEL_CUDA(m, cudaMemcpyAsync(grad, d_g, sizeof(double) * 3 * n, cudaMemcpyDeviceToHost, m->stream));
-  FUEL_CUDA(m, cudaStreamSynchronize(m->stream));
-  return 0;
+  return st.download();
 }
 
 int fuelgpu_frontier_search(FuelMap* m, const double upd_min[3], const double upd_max[3],
@@ -668,16 +696,16 @@ int fuelgpu_frontier_clear_flags(FuelMap* m, int32_t n, const int32_t* addr) {
   FUEL_CUDA(m, cudaSetDevice(m->dev));
   for (int i = 0; i < n; ++i)
     if (addr[i] < 0 || addr[i] >= m->nvox) return fuel_fail(m, FUELGPU_EINVAL, "address out of range");
-  // own small allocation: m->stage belongs to the main-stream ingest path
-  int* d_addr = nullptr;
-  FUEL_CUDA(m, cudaMalloc(&d_addr, sizeof(int) * (size_t)n));
+  // the frontier stream's scratch: m->stage belongs to the main-stream ingest path
+  int rc = m->fr_scr.ensure(m, sizeof(int) * (size_t)n);
+  if (rc) return rc;
+  int* d_addr = (int*)m->fr_scr.p;
   cudaStream_t fs = frontier_stream(m);
   FUEL_CUDA(m, cudaMemcpyAsync(d_addr, addr, sizeof(int) * n, cudaMemcpyHostToDevice, fs));
   clear_flags_kernel<<<(n + 255) / 256, 256, 0, fs>>>(m->flag, d_addr, n);
   FUEL_LAUNCHES(m, 1);
   FUEL_CUDA(m, cudaGetLastError());
   FUEL_CUDA(m, cudaStreamSynchronize(fs));
-  cudaFree(d_addr);
   return 0;
 }
 
@@ -821,18 +849,18 @@ int fuelgpu_bspline_cost_batch(FuelMap* m, int32_t B, int32_t n_pts, int32_t mas
   const size_t xb = sizeof(double) * (size_t)B * nvar;
   const size_t packb = ((offsetof(FuelTrajConst, guide) + sizeof(int32_t)) * (size_t)B + 63) & ~(size_t)63;
   const size_t fb = sizeof(double) * (size_t)B;
-  rc = ensure_bs(m, tcb + 2 * xb + fb + packb + 64);
+  rc = m->bs_buf.ensure(m, tcb + 2 * xb + fb + packb + 64);
   if (rc) return rc;
-  rc = ensure_bs_pin(m, packb + 2 * xb + fb);
+  rc = m->bs_pin.ensure(m, packb + 2 * xb + fb);
   if (rc) return rc;
-  uint8_t* base = (uint8_t*)m->bs_buf;
+  uint8_t* base = m->bs_buf.p;
   FuelTrajConst* d_tc = (FuelTrajConst*)base;
   double* d_x = (double*)(base + tcb);
   double* d_g = d_x + (size_t)B * nvar;
   double* d_f = d_g + (size_t)B * nvar;
   uint8_t* d_pack = (uint8_t*)(d_f + B);
   // host buffers of unknown provenance (pageable or pinned) bounce through the page-locked area
-  uint8_t* pin = (uint8_t*)m->bs_pin;
+  uint8_t* pin = m->bs_pin.p;
   double* h_x = (double*)(pin + packb);
   double* h_g = h_x + (size_t)B * nvar;
   double* h_f = h_g + (size_t)B * nvar;
@@ -888,18 +916,18 @@ int fuelgpu_bspline_optimize_batch_begin(FuelMap* m, int32_t B, int32_t n_pts, i
   const size_t xb = sizeof(double) * (size_t)B * nvar;
   const size_t packb = ((offsetof(FuelTrajConst, guide) + sizeof(int32_t)) * (size_t)B + 63) & ~(size_t)63;
   const size_t fb = sizeof(double) * (size_t)B, nb = sizeof(int32_t) * (size_t)B;
-  rc = ensure_bs(m, tcb + xb + fb + nb + packb + 64);
+  rc = m->bs_buf.ensure(m, tcb + xb + fb + nb + packb + 64);
   if (rc) return rc;
-  rc = ensure_bs_pin(m, packb + xb + fb + nb);
+  rc = m->bs_pin.ensure(m, packb + xb + fb + nb);
   if (rc) return rc;
-  uint8_t* base = (uint8_t*)m->bs_buf;
+  uint8_t* base = m->bs_buf.p;
   FuelTrajConst* d_tc = (FuelTrajConst*)base;
   double* d_x = (double*)(base + tcb);
   double* d_f = d_x + (size_t)B * nvar;
   int32_t* d_n = (int32_t*)(d_f + B);
   uint8_t* d_pack = (uint8_t*)(((uintptr_t)(d_n + B) + 63) & ~(uintptr_t)63);
   // host buffers of unknown provenance (pageable or pinned) bounce through the page-locked area
-  uint8_t* pin = (uint8_t*)m->bs_pin;
+  uint8_t* pin = m->bs_pin.p;
   double* h_x = (double*)(pin + packb);  // x, f_best, n_eval adjacent on both sides: one DMA back
   if (mask & FUELGPU_VIEWCONS)
     for (int b = 0; b < B; ++b)
@@ -936,7 +964,7 @@ int fuelgpu_bspline_optimize_batch_end(FuelMap* m, double* x, double* f_best, in
   m->bs_pend_B = 0;
   FUEL_CUDA(m, cudaSetDevice(m->dev));
   FUEL_CUDA(m, cudaStreamSynchronize(m->stream));
-  const uint8_t* h = (const uint8_t*)m->bs_pin + m->bs_pend_off;
+  const uint8_t* h = m->bs_pin.p + m->bs_pend_off;
   memcpy(x, h, xb);
   memcpy(f_best, h + xb, fb);
   memcpy(n_eval, h + xb + fb, nb);
@@ -968,18 +996,6 @@ static int check_traj_args(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar, b
   return 0;
 }
 
-static int ensure_tc(FuelMap* m, size_t bytes) {
-  if (bytes <= m->tc_bytes) return 0;
-  if (m->tc_buf) cudaFree(m->tc_buf);
-  m->tc_buf = nullptr;
-  m->tc_bytes = 0;
-  FUEL_CUDA(m, cudaMalloc(&m->tc_buf, bytes));
-  m->tc_bytes = bytes;
-  return 0;
-}
-
-static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
-
 int fuelgpu_bspline_check_batch_dev(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar, const void* x_dev,
                                     const void* dt_dev, const FuelTrajCheckParams* p, void* report_dev, void* best_dev) {
   int rc = check_traj_args(m, B, n_pts, nvar, x_dev != nullptr, dt_dev != nullptr);
@@ -999,28 +1015,18 @@ int fuelgpu_bspline_check_batch(FuelMap* m, int32_t B, int32_t n_pts, int32_t nv
   if (rc) return rc;
   if (!p || !best || (B > 0 && !report)) return fuel_fail(m, FUELGPU_EINVAL, "null argument");
   FUEL_CUDA(m, cudaSetDevice(m->dev));
-  const size_t xb = align256(sizeof(double) * (size_t)B * nvar), db = align256(sizeof(double) * (size_t)B);
-  const size_t rb = align256(sizeof(FuelTrajReport) * (size_t)B);
-  rc = ensure_tc(m, xb + db + rb + 256);
+  double *d_x, *d_dt;
+  FuelTrajReport* d_rep;
+  int32_t* d_best;
+  HostStaging st(m);
+  st.in(&d_x, x, (size_t)B * nvar).in(&d_dt, dt, (size_t)B).out(&d_rep, report, (size_t)B).out(&d_best, best, 2);
+  rc = st.upload();
   if (rc) return rc;
-  uint8_t* base = (uint8_t*)m->tc_buf;
-  double* d_x = (double*)base;
-  double* d_dt = dt ? (double*)(base + xb) : nullptr;
-  FuelTrajReport* d_rep = (FuelTrajReport*)(base + xb + db);
-  int32_t* d_best = (int32_t*)(base + xb + db + rb);
-  if (B > 0) {
-    FUEL_CUDA(m, cudaMemcpyAsync(d_x, x, sizeof(double) * (size_t)B * nvar, cudaMemcpyHostToDevice, m->stream));
-    if (dt) FUEL_CUDA(m, cudaMemcpyAsync(d_dt, dt, sizeof(double) * (size_t)B, cudaMemcpyHostToDevice, m->stream));
-  }
   tbegin(m, T_CHECK);
   rc = traj_check_impl(m, B, n_pts, nvar, d_x, d_dt, p, d_rep, d_best);
   tend(m, T_CHECK);
   if (rc) return rc;
-  if (B > 0)
-    FUEL_CUDA(m, cudaMemcpyAsync(report, d_rep, sizeof(FuelTrajReport) * (size_t)B, cudaMemcpyDeviceToHost, m->stream));
-  FUEL_CUDA(m, cudaMemcpyAsync(best, d_best, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, m->stream));
-  FUEL_CUDA(m, cudaStreamSynchronize(m->stream));
-  return 0;
+  return st.download();
 }
 
 int fuelgpu_bspline_evaluate_batch(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar, const double* x, const double* dt,
@@ -1032,23 +1038,14 @@ int fuelgpu_bspline_evaluate_batch(FuelMap* m, int32_t B, int32_t n_pts, int32_t
   if (!t || !out) return fuel_fail(m, FUELGPU_EINVAL, "null argument");
   FUEL_CUDA(m, cudaSetDevice(m->dev));
   const size_t nt = (size_t)B * n_t;
-  const size_t xb = align256(sizeof(double) * (size_t)B * nvar), db = align256(sizeof(double) * (size_t)B);
-  const size_t tb = align256(sizeof(double) * nt);
-  rc = ensure_tc(m, xb + db + tb + sizeof(double) * 3 * nt);
+  double *d_x, *d_dt, *d_t, *d_out;
+  HostStaging st(m);
+  st.in(&d_x, x, (size_t)B * nvar).in(&d_dt, dt, (size_t)B).in(&d_t, t, nt).out(&d_out, out, 3 * nt);
+  rc = st.upload();
   if (rc) return rc;
-  uint8_t* base = (uint8_t*)m->tc_buf;
-  double* d_x = (double*)base;
-  double* d_dt = dt ? (double*)(base + xb) : nullptr;
-  double* d_t = (double*)(base + xb + db);
-  double* d_out = (double*)(base + xb + db + tb);
-  FUEL_CUDA(m, cudaMemcpyAsync(d_x, x, sizeof(double) * (size_t)B * nvar, cudaMemcpyHostToDevice, m->stream));
-  if (dt) FUEL_CUDA(m, cudaMemcpyAsync(d_dt, dt, sizeof(double) * (size_t)B, cudaMemcpyHostToDevice, m->stream));
-  FUEL_CUDA(m, cudaMemcpyAsync(d_t, t, sizeof(double) * nt, cudaMemcpyHostToDevice, m->stream));
   rc = traj_evaluate_impl(m, B, n_pts, nvar, d_x, d_dt, n_t, d_t, deriv, d_out);
   if (rc) return rc;
-  FUEL_CUDA(m, cudaMemcpyAsync(out, d_out, sizeof(double) * 3 * nt, cudaMemcpyDeviceToHost, m->stream));
-  FUEL_CUDA(m, cudaStreamSynchronize(m->stream));
-  return 0;
+  return st.download();
 }
 
 static int check_param_args(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar, const void* points, const void* derivs,
@@ -1084,30 +1081,19 @@ int fuelgpu_bspline_parameterize_batch(FuelMap* m, int32_t B, int32_t n_pts, int
       return fuel_fail(m, FUELGPU_EINVAL, "dt[%s%lld] must be finite and positive", "", (long long)b);
   if (B == 0) return 0;
   FUEL_CUDA(m, cudaSetDevice(m->dev));
-  const size_t K = (size_t)n_pts - 2;
-  const size_t pb = align256(sizeof(double) * B * K * 3), gb = align256(sizeof(double) * B * 12);
-  const size_t db = align256(sizeof(double) * B), xb = align256(sizeof(double) * B * nvar);
-  rc = ensure_tc(m, pb + gb + 2 * db + xb + sizeof(FuelTrajConst) * B);
+  const size_t nb = (size_t)B, K = (size_t)n_pts - 2;
+  double *d_pts, *d_der, *d_dt, *d_tlb, *d_x;
+  FuelTrajConst* d_tc;
+  HostStaging st(m);
+  st.in(&d_pts, points, nb * K * 3).in(&d_der, derivs, nb * 12).in(&d_dt, dt, nb).in(&d_tlb, time_lb, nb);
+  st.out(&d_x, x, nb * nvar).out(&d_tc, traj, nb);
+  rc = st.upload();
   if (rc) return rc;
-  uint8_t* base = (uint8_t*)m->tc_buf;
-  double* d_pts = (double*)base;
-  double* d_der = (double*)(base + pb);
-  double* d_dt = (double*)(base + pb + gb);
-  double* d_tlb = time_lb ? (double*)(base + pb + gb + db) : nullptr;
-  double* d_x = (double*)(base + pb + gb + 2 * db);
-  FuelTrajConst* d_tc = (FuelTrajConst*)(base + pb + gb + 2 * db + xb);
-  FUEL_CUDA(m, cudaMemcpyAsync(d_pts, points, sizeof(double) * B * K * 3, cudaMemcpyHostToDevice, m->stream));
-  FUEL_CUDA(m, cudaMemcpyAsync(d_der, derivs, sizeof(double) * B * 12, cudaMemcpyHostToDevice, m->stream));
-  FUEL_CUDA(m, cudaMemcpyAsync(d_dt, dt, sizeof(double) * B, cudaMemcpyHostToDevice, m->stream));
-  if (time_lb) FUEL_CUDA(m, cudaMemcpyAsync(d_tlb, time_lb, sizeof(double) * B, cudaMemcpyHostToDevice, m->stream));
   tbegin(m, T_PARAM);
   rc = traj_param_impl(m, B, n_pts, nvar, d_pts, d_der, d_dt, d_tlb, d_x, d_tc);
   tend(m, T_PARAM);
   if (rc) return rc;
-  FUEL_CUDA(m, cudaMemcpyAsync(x, d_x, sizeof(double) * B * nvar, cudaMemcpyDeviceToHost, m->stream));
-  FUEL_CUDA(m, cudaMemcpyAsync(traj, d_tc, sizeof(FuelTrajConst) * B, cudaMemcpyDeviceToHost, m->stream));
-  FUEL_CUDA(m, cudaStreamSynchronize(m->stream));
-  return 0;
+  return st.download();
 }
 
 
@@ -1172,48 +1158,21 @@ int fuelgpu_poly_waypoints_batch(FuelMap* m, int32_t B, int32_t w_max, const int
   }
   if (B == 0) return 0;
   FUEL_CUDA(m, cudaSetDevice(m->dev));
-  const size_t S1 = (size_t)w_max - 1, K = FUELGPU_MAX_PTS - 2;
-  const size_t nb = align256(sizeof(int32_t) * B), wb = align256(sizeof(double) * B * w_max * 3);
-  const size_t vb = align256(sizeof(double) * B * 3), tb = times ? align256(sizeof(double) * B * S1) : 0;
-  const size_t ib = align256(sizeof(FuelPolyInfo) * B), cb = coeffs ? align256(sizeof(double) * B * S1 * 18) : 0;
-  const size_t pb = align256(sizeof(double) * B * K * 3), db = align256(sizeof(double) * B * 12);
-  rc = ensure_tc(m, nb + wb + 4 * vb + tb + ib + cb + pb + db);
+  const size_t nb = (size_t)B, S1 = (size_t)w_max - 1, K = FUELGPU_MAX_PTS - 2;
+  int32_t* d_n;
+  double *d_wp, *d_sv, *d_sa, *d_ev, *d_ea, *d_t, *d_c, *d_p, *d_d;
+  FuelPolyInfo* d_info;
+  HostStaging st(m);
+  st.in(&d_n, n_wp, nb).in(&d_wp, waypts, nb * w_max * 3).in(&d_sv, start_vel, nb * 3).in(&d_sa, start_acc, nb * 3);
+  st.in(&d_ev, end_vel, nb * 3).in(&d_ea, end_acc, nb * 3).in(&d_t, times, nb * S1);
+  st.out(&d_info, info, nb).out(&d_c, coeffs, nb * S1 * 18).out(&d_p, points, nb * K * 3).out(&d_d, derivs, nb * 12);
+  rc = st.upload();
   if (rc) return rc;
-  uint8_t* q = (uint8_t*)m->tc_buf;
-  int32_t* d_n = (int32_t*)q;
-  q += nb;
-  double* d_wp = (double*)q;
-  q += wb;
-  double* d_sv = (double*)q;
-  double* d_sa = (double*)(q + vb);
-  double* d_ev = end_vel ? (double*)(q + 2 * vb) : nullptr;
-  double* d_ea = end_acc ? (double*)(q + 3 * vb) : nullptr;
-  q += 4 * vb;
-  double* d_t = times ? (double*)q : nullptr;
-  q += tb;
-  FuelPolyInfo* d_info = (FuelPolyInfo*)q;
-  q += ib;
-  double* d_c = coeffs ? (double*)q : nullptr;
-  q += cb;
-  double* d_p = (double*)q;
-  double* d_d = (double*)(q + pb);
-  FUEL_CUDA(m, cudaMemcpyAsync(d_n, n_wp, sizeof(int32_t) * B, cudaMemcpyHostToDevice, m->stream));
-  FUEL_CUDA(m, cudaMemcpyAsync(d_wp, waypts, sizeof(double) * B * w_max * 3, cudaMemcpyHostToDevice, m->stream));
-  FUEL_CUDA(m, cudaMemcpyAsync(d_sv, start_vel, sizeof(double) * B * 3, cudaMemcpyHostToDevice, m->stream));
-  FUEL_CUDA(m, cudaMemcpyAsync(d_sa, start_acc, sizeof(double) * B * 3, cudaMemcpyHostToDevice, m->stream));
-  if (end_vel) FUEL_CUDA(m, cudaMemcpyAsync(d_ev, end_vel, sizeof(double) * B * 3, cudaMemcpyHostToDevice, m->stream));
-  if (end_acc) FUEL_CUDA(m, cudaMemcpyAsync(d_ea, end_acc, sizeof(double) * B * 3, cudaMemcpyHostToDevice, m->stream));
-  if (times) FUEL_CUDA(m, cudaMemcpyAsync(d_t, times, sizeof(double) * B * S1, cudaMemcpyHostToDevice, m->stream));
   tbegin(m, T_POLY);
   rc = poly_waypoints_impl(m, B, w_max, d_n, d_wp, d_sv, d_sa, d_ev, d_ea, d_t, p, d_info, d_c, d_p, d_d);
   tend(m, T_POLY);
   if (rc) return rc;
-  FUEL_CUDA(m, cudaMemcpyAsync(info, d_info, sizeof(FuelPolyInfo) * B, cudaMemcpyDeviceToHost, m->stream));
-  if (coeffs) FUEL_CUDA(m, cudaMemcpyAsync(coeffs, d_c, sizeof(double) * B * S1 * 18, cudaMemcpyDeviceToHost, m->stream));
-  FUEL_CUDA(m, cudaMemcpyAsync(points, d_p, sizeof(double) * B * K * 3, cudaMemcpyDeviceToHost, m->stream));
-  FUEL_CUDA(m, cudaMemcpyAsync(derivs, d_d, sizeof(double) * B * 12, cudaMemcpyDeviceToHost, m->stream));
-  FUEL_CUDA(m, cudaStreamSynchronize(m->stream));
-  return 0;
+  return st.download();
 }
 
 static int check_yaw_args(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar, const void* x, const void* dt,
@@ -1259,33 +1218,17 @@ int fuelgpu_yaw_explore_batch(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar
   }
   if (B == 0) return 0;
   FUEL_CUDA(m, cudaSetDevice(m->dev));
-  const size_t xb = align256(sizeof(double) * B * nvar), db = align256(sizeof(double) * B);
-  const size_t sb = align256(sizeof(double) * B * 3), yb = align256(sizeof(double) * B * FUELGPU_YAW_PTS);
-  const size_t ib = align256(sizeof(FuelYawInfo) * B), wb = sizeof(double) * B * FUELGPU_YAW_MAX_WAYPT;
-  rc = ensure_tc(m, xb + 2 * db + sb + yb + ib + wb);
+  const size_t nb = (size_t)B;
+  double *d_x, *d_dt, *d_sy, *d_ey, *d_yaw, *d_wp;
+  FuelYawInfo* d_info;
+  HostStaging st(m);
+  st.in(&d_x, x, nb * nvar).in(&d_dt, dt, nb).in(&d_sy, start_yaw, nb * 3).in(&d_ey, end_yaw, nb);
+  st.out(&d_yaw, yaw, nb * FUELGPU_YAW_PTS).out(&d_info, info, nb).out(&d_wp, waypt, nb * FUELGPU_YAW_MAX_WAYPT);
+  rc = st.upload();
   if (rc) return rc;
-  uint8_t* q = (uint8_t*)m->tc_buf;
-  double* d_x = (double*)q;
-  double* d_dt = dt ? (double*)(q + xb) : nullptr;
-  double* d_ey = (double*)(q + xb + db);
-  q += xb + 2 * db;
-  double* d_sy = (double*)q;
-  double* d_yaw = (double*)(q + sb);
-  FuelYawInfo* d_info = (FuelYawInfo*)(q + sb + yb);
-  double* d_wp = waypt ? (double*)(q + sb + yb + ib) : nullptr;
-  FUEL_CUDA(m, cudaMemcpyAsync(d_x, x, sizeof(double) * B * nvar, cudaMemcpyHostToDevice, m->stream));
-  if (dt) FUEL_CUDA(m, cudaMemcpyAsync(d_dt, dt, sizeof(double) * B, cudaMemcpyHostToDevice, m->stream));
-  FUEL_CUDA(m, cudaMemcpyAsync(d_sy, start_yaw, sizeof(double) * B * 3, cudaMemcpyHostToDevice, m->stream));
-  FUEL_CUDA(m, cudaMemcpyAsync(d_ey, end_yaw, sizeof(double) * B, cudaMemcpyHostToDevice, m->stream));
   rc = yaw_explore_impl(m, B, n_pts, nvar, d_x, d_dt, d_sy, d_ey, p, yp, d_yaw, d_info, d_wp);
   if (rc) return rc;
-  FUEL_CUDA(m, cudaMemcpyAsync(yaw, d_yaw, sizeof(double) * B * FUELGPU_YAW_PTS, cudaMemcpyDeviceToHost, m->stream));
-  FUEL_CUDA(m, cudaMemcpyAsync(info, d_info, sizeof(FuelYawInfo) * B, cudaMemcpyDeviceToHost, m->stream));
-  if (waypt)
-    FUEL_CUDA(m, cudaMemcpyAsync(waypt, d_wp, sizeof(double) * B * FUELGPU_YAW_MAX_WAYPT, cudaMemcpyDeviceToHost,
-                                 m->stream));
-  FUEL_CUDA(m, cudaStreamSynchronize(m->stream));
-  return 0;
+  return st.download();
 }
 
 static int check_astar_args(FuelMap* m, int32_t B, const void* start, const void* goal, const FuelAstarParams* p,
@@ -1328,30 +1271,18 @@ int fuelgpu_astar_batch(FuelMap* m, int32_t B, const double* start, const double
         return fuel_fail(m, FUELGPU_EINVAL, "query %s%lld: start and goal must be finite", "", (long long)b);
   if (B == 0) return 0;
   FUEL_CUDA(m, cudaSetDevice(m->dev));
-  const size_t vb = align256(sizeof(double) * B * 3), ib = align256(sizeof(FuelPathInfo) * B);
-  const size_t pb = path ? align256(sizeof(double) * B * (size_t)path_max * 3) : 0;
-  const size_t nb = align256(sizeof(int32_t) * B), wb = sizeof(double) * B * (size_t)w_max * 3;
-  rc = ensure_tc(m, 2 * vb + ib + pb + nb + wb);
+  const size_t nb = (size_t)B;
+  double *d_s, *d_g, *d_path, *d_wp;
+  FuelPathInfo* d_info;
+  int32_t* d_n;
+  HostStaging st(m);
+  st.in(&d_s, start, nb * 3).in(&d_g, goal, nb * 3).out(&d_info, info, nb);
+  st.out(&d_path, path, nb * path_max * 3).out(&d_n, n_wp, nb).out(&d_wp, waypts, nb * w_max * 3);
+  rc = st.upload();
   if (rc) return rc;
-  uint8_t* q = (uint8_t*)m->tc_buf;
-  double* d_s = (double*)q;
-  double* d_g = (double*)(q + vb);
-  FuelPathInfo* d_info = (FuelPathInfo*)(q + 2 * vb);
-  double* d_path = path ? (double*)(q + 2 * vb + ib) : nullptr;
-  int32_t* d_n = (int32_t*)(q + 2 * vb + ib + pb);
-  double* d_wp = (double*)(q + 2 * vb + ib + pb + nb);
-  FUEL_CUDA(m, cudaMemcpyAsync(d_s, start, sizeof(double) * B * 3, cudaMemcpyHostToDevice, m->stream));
-  FUEL_CUDA(m, cudaMemcpyAsync(d_g, goal, sizeof(double) * B * 3, cudaMemcpyHostToDevice, m->stream));
   rc = astar_impl(m, B, d_s, d_g, p, d_info, path_max, d_path, w_max, d_n, d_wp);
   if (rc) return rc;
-  FUEL_CUDA(m, cudaMemcpyAsync(info, d_info, sizeof(FuelPathInfo) * B, cudaMemcpyDeviceToHost, m->stream));
-  if (path)
-    FUEL_CUDA(m, cudaMemcpyAsync(path, d_path, sizeof(double) * B * (size_t)path_max * 3, cudaMemcpyDeviceToHost,
-                                 m->stream));
-  FUEL_CUDA(m, cudaMemcpyAsync(n_wp, d_n, sizeof(int32_t) * B, cudaMemcpyDeviceToHost, m->stream));
-  FUEL_CUDA(m, cudaMemcpyAsync(waypts, d_wp, wb, cudaMemcpyDeviceToHost, m->stream));
-  FUEL_CUDA(m, cudaStreamSynchronize(m->stream));
-  return 0;
+  return st.download();
 }
 
 }  // extern "C"

@@ -465,20 +465,13 @@ int astar_impl(FuelMap* m, int B, const double* start_dev, const double* goal_de
   W = std::min(W, (size_t)m->sm_count * 32);
   W = std::min(W, std::max((size_t)1, AS_BUDGET / c.stride));
   const size_t blocks = (W + AS_WARPS - 1) / AS_WARPS, warps = blocks * AS_WARPS;
-  const size_t bytes = 256 + warps * c.stride;
-  if (bytes > m->as_bytes) {
-    if (m->as_buf) cudaFree(m->as_buf);
-    m->as_buf = nullptr;
-    m->as_bytes = 0;
-    m->as_stride = 0;
-    m->as_warps = 0;
-    FUEL_CUDA(m, cudaMalloc(&m->as_buf, bytes));
-    m->as_bytes = bytes;
-  }
-  uint8_t* scr = (uint8_t*)m->as_buf + 256;
+  bool fresh = false;
+  const int rc = m->as_buf.ensure(m, 256 + warps * c.stride, &fresh);
+  if (rc) return rc;
+  uint8_t* scr = m->as_buf.p + 256;
   // every key table starts empty (all bits set); a search clears the slots it used before it ends, so only a new
-  // layout or warps not used before need the fill
-  if (m->as_stride != c.stride) {
+  // block, a new layout or warps not used before need the fill
+  if (fresh || m->as_stride != c.stride) {
     FUEL_CUDA(m, cudaMemsetAsync(scr, 0xff, warps * c.stride, m->stream));
     m->as_stride = c.stride;
     m->as_warps = warps;
@@ -486,7 +479,7 @@ int astar_impl(FuelMap* m, int B, const double* start_dev, const double* goal_de
     FUEL_CUDA(m, cudaMemsetAsync(scr + m->as_warps * c.stride, 0xff, (warps - m->as_warps) * c.stride, m->stream));
     m->as_warps = warps;
   }
-  int* counter = (int*)m->as_buf;
+  int* counter = (int*)m->as_buf.p;
   FUEL_CUDA(m, cudaMemsetAsync(counter, 0, sizeof(int), m->stream));
   astar_kernel<<<(unsigned)blocks, AS_THREADS, 0, m->stream>>>(m->g, m->occ, c, B, start_dev, goal_dev, scr, counter,
                                                               info_dev, path_dev, nwp_dev, wp_dev);

@@ -677,16 +677,6 @@ __global__ void __launch_bounds__(SOLVER_WPB * 32, SOLVER_SM_WARPS / SOLVER_WPB)
 #endif
 }
 
-int ensure_bs_grad(FuelMap* m, size_t bytes) {  // freed with the map (fuelgpu_map_destroy)
-  if (bytes <= m->bs_grad_bytes) return 0;
-  if (m->bs_grad) cudaFree(m->bs_grad);
-  m->bs_grad = nullptr;
-  m->bs_grad_bytes = 0;
-  FUEL_CUDA(m, cudaMalloc(&m->bs_grad, bytes));
-  m->bs_grad_bytes = bytes;
-  return 0;
-}
-
 }  // namespace
 
 // The solver kernels write best_variable_ and the evaluation count; min_cost_ at the returned x then comes from the
@@ -697,7 +687,7 @@ int bspline_optimize_batch_dev_impl(FuelMap* m, int B, int n_pts, int mask, cons
                                     double* x_dev, double* fbest_dev, int32_t* neval_dev) {
   if (B <= 0) return 0;
   const int nvar = (mask & FUELGPU_MINTIME) ? 3 * n_pts + 1 : 3 * n_pts;
-  int rc = ensure_bs_grad(m, sizeof(double) * (size_t)B * nvar);
+  int rc = m->bs_grad.ensure(m, (size_t)B * nvar);
   if (rc) return rc;
   static int use_vec = -1;  // FUELGPU_SOLVER=vec selects the vector-space two-loop recursion (A/B, debugging)
   if (use_vec < 0) {
@@ -724,7 +714,7 @@ int bspline_optimize_batch_dev_impl(FuelMap* m, int B, int n_pts, int mask, cons
     FUEL_CUDA(m, cudaGetLastError());
   }
   return bspline_cost_batch_dev_impl(m, B, n_pts, mask & ~FUELGPU_COST_FAST_EVAL, p, tc_dev, x_dev, fbest_dev,
-                                     (double*)m->bs_grad);
+                                     m->bs_grad.p);
 }
 
 #ifdef FUEL_PROF

@@ -27,6 +27,22 @@ enum { T_ESDF = 0, T_FRONTIER = 1, T_BSPLINE = 2, T_UPLOAD = 3, T_DOWNLOAD = 4, 
 
 struct FrontierState;  // frontier.cu
 struct FusionState;    // fusion.cu
+struct FuelMap;
+
+// A scratch block that grows on demand: device memory, or page-locked host memory when Pinned.  Growing first waits
+// for the whole device, since any stream may still use the old block; steady-state calls never wait.
+template <typename T, bool Pinned = false>
+struct DevBuf {
+  T* p = nullptr;
+  size_t cap = 0;  // elements
+  // at least n elements at p; *grew (if given) tells whether the block was replaced (its contents are then undefined)
+  int ensure(FuelMap* m, size_t n, bool* grew = nullptr);
+  void release() {
+    if (p) Pinned ? cudaFreeHost(p) : cudaFree(p);
+    p = nullptr;
+    cap = 0;
+  }
+};
 
 struct FuelMap {
   FuelGridDesc desc;
@@ -45,9 +61,9 @@ struct FuelMap {
   size_t esdf_p_bytes;
   cudaStream_t esdf_aux;
   cudaEvent_t esdf_ev[2];
-  // staging for ingest
-  void* stage;
-  size_t stage_bytes;
+  // Grow-on-demand scratch.  Each block belongs to one stream (or one pending call); calls that may overlap never
+  // share a block.
+  DevBuf<uint8_t> stage;  // main-stream ingest and downloads
   cudaStream_t own_stream, stream;
   cudaStream_t copy_stream;  // D2H mirror copies that may overlap the main stream
   cudaEvent_t copy_ev;
@@ -58,23 +74,16 @@ struct FuelMap {
   bool ev_valid[T_COUNT];
   FrontierState* fs;
   FusionState* fus;  // lazily created by the first fusion call
-  // bspline scratch (device)
-  void* bs_buf;
-  size_t bs_bytes;
-  void* bs_pin;  // page-locked bounce buffer for the host-facing B-spline calls
-  size_t bs_pin_bytes;
-  void* bs_grad;  // gradient output of the faithful re-evaluation after the long-trajectory solver (discarded)
-  size_t bs_grad_bytes;
-  void* fr_scr;  // device scratch of the small frontier-side calls (is_changed, viewpoints), grown on demand
-  size_t fr_scr_bytes;
+  DevBuf<uint8_t> bs_buf;       // host-facing cost / optimize calls (owned by a pending optimize_batch_begin)
+  DevBuf<uint8_t, true> bs_pin;  // their page-locked bounce buffer
+  DevBuf<double> bs_grad;  // gradient output of the faithful re-evaluation after the long-trajectory solver (discarded)
+  DevBuf<uint8_t> fr_scr;  // small frontier-stream calls (is_changed, viewpoints, clear_flags)
   int bs_pend_B, bs_pend_nvar;  // optimize_batch_begin issued, _end outstanding (B == 0: none)
   size_t bs_pend_off;           // offset of the result block inside bs_pin
   long long launches;  // kernels launched so far
   char err[512];
-  void* tc_buf;  // device scratch of the host-facing trajectory check / evaluate calls, grown on demand
-  size_t tc_bytes;
-  void* as_buf;  // A* search scratch (astar.cu), grown on demand
-  size_t as_bytes;
+  DevBuf<uint8_t> tc_buf;  // the other host-facing batch calls (check, evaluate, parameterize, poly, yaw, A*, esdf_sample)
+  DevBuf<uint8_t> as_buf;  // A* search scratch (astar.cu)
   size_t as_stride, as_warps;  // layout whose key tables are known empty: per-warp bytes, warps
 };
 
@@ -96,6 +105,23 @@ static inline int fuel_fail(FuelMap* m, int code, const char* fmt, const char* a
       return _e == cudaErrorMemoryAllocation ? FUELGPU_ENOMEM : FUELGPU_ECUDA;                 \
     }                                                                                          \
   } while (0)
+
+template <typename T, bool Pinned>
+int DevBuf<T, Pinned>::ensure(FuelMap* m, size_t n, bool* grew) {
+  if (grew) *grew = false;
+  if (n <= cap) return 0;
+  if (p) {
+    FUEL_CUDA(m, cudaDeviceSynchronize());
+    release();
+  }
+  const size_t want = n + n / 4 + 1024;
+  T* q = nullptr;
+  FUEL_CUDA(m, Pinned ? cudaMallocHost((void**)&q, want * sizeof(T)) : cudaMalloc((void**)&q, want * sizeof(T)));
+  p = q;
+  cap = want;
+  if (grew) *grew = true;
+  return 0;
+}
 
 static inline void tbegin(FuelMap* m, int t, cudaStream_t s = nullptr) { cudaEventRecord(m->ev0[t], s ? s : m->stream); }
 static inline void tend(FuelMap* m, int t, cudaStream_t s = nullptr) {
@@ -143,7 +169,6 @@ int frontier_search_from_candidates_impl(FuelMap* m, const double umin[3], const
                                          int32_t n, const int32_t* addr, const uint8_t* cls, int32_t* n_clusters,
                                          int32_t* n_cells, int32_t* n_filtered);  // main-stream writers of `occ` wait for an enqueued frontier search
 
-int ensure_fr_scratch(FuelMap* m, size_t bytes);
 int frontier_state_create(FuelMap* m);
 // The frontier subsystem runs on its own stream (it only reads `occ` and owns `flag`), so a host
 // thread can search frontiers while another updates the ESDF / runs the B-spline batch on the

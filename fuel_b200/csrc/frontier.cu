@@ -1486,42 +1486,6 @@ __global__ void is_changed_kernel(Geom g, const uint8_t* __restrict__ occ, const
   }
 }
 
-template <typename T>
-struct DevBuf {
-  T* p = nullptr;
-  size_t cap = 0;
-  int ensure(size_t n) {
-    if (n <= cap) return 0;
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-    size_t want = n + n / 4 + 1024;
-    if (cudaMalloc(&p, want * sizeof(T)) != cudaSuccess) return FUELGPU_ENOMEM;
-    cap = want;
-    return 0;
-  }
-  // grow keeping the first `keep` elements (stream-ordered copy on `s`)
-  int grow_preserve(size_t n, size_t keep, cudaStream_t s) {
-    if (n <= cap) return 0;
-    T* np = nullptr;
-    size_t want = n + n / 2 + 1024;
-    if (cudaMalloc(&np, want * sizeof(T)) != cudaSuccess) return FUELGPU_ENOMEM;
-    if (p && keep) {
-      cudaMemcpyAsync(np, p, keep * sizeof(T), cudaMemcpyDeviceToDevice, s);
-      cudaStreamSynchronize(s);
-    }
-    if (p) cudaFree(p);
-    p = np;
-    cap = want;
-    return 0;
-  }
-  void release() {
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-  }
-};
-
 }  // namespace
 
 struct SweepPlan {  // how the voxel sweep of a search is laid out
@@ -1560,8 +1524,7 @@ struct FrontierState {
   cudaEvent_t ev_in = nullptr;
   cudaEvent_t ev_out = nullptr;  // end of the last enqueued search: writers of `occ` on the main stream wait for it
   bool ev_out_valid = false;
-  char* h_pin = nullptr;  // pinned host staging for the result download
-  size_t h_pin_bytes = 0;
+  DevBuf<char, true> h_pin;  // pinned host staging for the result download
   int* d_counters = nullptr;  // [0] n_cand [1] n_roots [2] n_kept [3] n_new [4] small-path status [5] C
   // results of the last search (host side, CSR)
   std::vector<int32_t> h_cell_off, h_cell_addr, h_filt_off;
@@ -1605,15 +1568,15 @@ int frontier_state_create(FuelMap* m) {
 void frontier_state_destroy(FuelMap* m) {
   if (!m->fs) return;
   FrontierState* f = m->fs;
-  if (f->cellidx) cudaFree(f->cellidx);
-  if (f->d_counters) cudaFree(f->d_counters);
-  if (f->h_pin) cudaFreeHost(f->h_pin);
   if (f->stream) {
     cudaStreamSynchronize(f->stream);
     cudaStreamDestroy(f->stream);
   }
   if (f->ev_in) cudaEventDestroy(f->ev_in);
   if (f->ev_out) cudaEventDestroy(f->ev_out);
+  if (f->cellidx) cudaFree(f->cellidx);
+  if (f->d_counters) cudaFree(f->d_counters);
+  f->h_pin.release();
   f->maskE.release(); f->maskS.release(); f->blockcnt.release(); f->blockoff.release();
   f->scan_tot.release(); f->scan_off.release();
   f->cell_addr.release(); f->parent.release(); f->claim.release(); f->csize.release();
@@ -1624,9 +1587,10 @@ void frontier_state_destroy(FuelMap* m) {
   m->fs = nullptr;
 }
 
-#define ENSURE(buf, n)                                         \
-  do {                                                         \
-    if ((buf).ensure(n)) return fuel_fail(m, FUELGPU_ENOMEM, "frontier: device allocation failed"); \
+#define ENSURE(buf, n)                      \
+  do {                                      \
+    const int _rc = (buf).ensure(m, (n));   \
+    if (_rc) return _rc;                    \
   } while (0)
 
 static inline unsigned nblk(int64_t n, int b) { return (unsigned)((n + b - 1) / b); }
@@ -1641,8 +1605,8 @@ static int scan_ints(FuelMap* m, const int* in, int* out, int n, int* total) {
     return 0;
   }
   const int nchunk = (n + 1023) / 1024;
-  if (f->scan_tot.ensure(nchunk) || f->scan_off.ensure(nchunk))
-    return fuel_fail(m, FUELGPU_ENOMEM, "frontier: device allocation failed");
+  ENSURE(f->scan_tot, nchunk);
+  ENSURE(f->scan_off, nchunk);
   scan_chunks_kernel<<<nchunk, 1024, 0, s>>>(in, out, n, f->scan_tot.p);
   scan_kernel<<<1, 1024, 0, s>>>(f->scan_tot.p, f->scan_off.p, nchunk, total);
   scan_add_kernel<<<nchunk, 1024, 0, s>>>(out, n, f->scan_off.p);
@@ -1700,17 +1664,6 @@ static void sweep_compact(FuelMap* m, const FParams& fp, const SweepPlan& pl, in
 
 static size_t view_bytes(int K, int C) {
   return (size_t)K * (3 * sizeof(int) + 3 * sizeof(float)) + (size_t)C * (sizeof(ClusterMeta) + sizeof(ClusterStat)) + 64;
-}
-
-static int ensure_pin(FuelMap* m, size_t bytes) {
-  FrontierState* f = m->fs;
-  if (bytes <= f->h_pin_bytes) return 0;
-  if (f->h_pin) cudaFreeHost(f->h_pin);
-  f->h_pin = nullptr;
-  f->h_pin_bytes = 0;
-  FUEL_CUDA(m, cudaMallocHost((void**)&f->h_pin, bytes));
-  f->h_pin_bytes = bytes;
-  return 0;
 }
 
 // byte offsets of the arrays of K cells / C clusters in a result buffer (16-byte aligned pieces)
@@ -1899,10 +1852,10 @@ static void frontier_apply_bfs_order(FuelMap* m, const std::vector<int>& out_roo
 
 static int frontier_marshal(FuelMap* m, int K, int C, int32_t* n_clusters, int32_t* n_cells,
                             int32_t* n_filtered) {
-  int rc = ensure_pin(m, view_bytes(K, C));
+  int rc = m->fs->h_pin.ensure(m, view_bytes(K, C));
   if (rc) return rc;
   HostView hv;
-  rc = enqueue_download(m, K, C, m->fs->h_pin, &hv);
+  rc = enqueue_download(m, K, C, m->fs->h_pin.p, &hv);
   if (rc) return rc;
   FUEL_CUDA(m, cudaStreamSynchronize(m->fs->stream));
   return frontier_build_csr(m, K, C, hv, n_clusters, n_cells, n_filtered);
@@ -2099,10 +2052,9 @@ int frontier_search_begin_impl(FuelMap* m, const double umin[3], const double um
     }
     cluster_small_kernel<<<SMALL_CTAS, 1024, 0, s>>>(g, fp, m->flag, f->cellidx, sb);
     FUEL_LAUNCHES(m, 1);
-    int rc0 = ensure_pin(m, 64 + rl.bytes);
-    if (rc0) return rc0;
-    FUEL_CUDA(m, cudaMemcpyAsync(f->h_pin, f->res.p, 64 + rl.bytes, cudaMemcpyDeviceToHost, s));
-    result_view(rl, f->h_pin + 64, &f->pend_hv);
+    ENSURE(f->h_pin, 64 + rl.bytes);
+    FUEL_CUDA(m, cudaMemcpyAsync(f->h_pin.p, f->res.p, 64 + rl.bytes, cudaMemcpyDeviceToHost, s));
+    result_view(rl, f->h_pin.p + 64, &f->pend_hv);
     f->pend_fp = fp;
     f->pend_plan = pl;
     f->pend_active = true;
@@ -2128,7 +2080,7 @@ int frontier_search_end_impl(FuelMap* m, int32_t* n_clusters, int32_t* n_cells, 
   const SweepPlan pl = f->pend_plan;
   int n_cand = 0;
   {
-    const int* cnt = (const int*)f->h_pin;
+    const int* cnt = (const int*)f->h_pin.p;
     HostView& hv = f->pend_hv;
     FUEL_CUDA(m, cudaStreamSynchronize(s));
     n_cand = cnt[0];
@@ -2337,28 +2289,14 @@ int frontier_fetch_impl(FuelMap* m, int32_t* cell_offsets, int32_t* cell_addr, i
   return 0;
 }
 
-int ensure_fr_scratch(FuelMap* m, size_t bytes) {
-  if (bytes <= m->fr_scr_bytes) return 0;
-  if (m->fr_scr) {
-    cudaDeviceSynchronize();  // both streams may still use the old block
-    cudaFree(m->fr_scr);
-  }
-  m->fr_scr = nullptr;
-  m->fr_scr_bytes = 0;
-  const size_t want = bytes + bytes / 2 + 4096;
-  FUEL_CUDA(m, cudaMalloc(&m->fr_scr, want));
-  m->fr_scr_bytes = want;
-  return 0;
-}
-
 int frontier_is_changed_impl(FuelMap* m, int32_t mcl, const int32_t* offs, const int32_t* addr,
                              uint8_t* changed, int32_t* counts) {
   if (mcl <= 0) return 0;
   const int ncell = offs[mcl];
   const size_t nci = (size_t)(ncell > 0 ? ncell : 1);
-  int rc = ensure_fr_scratch(m, sizeof(int) * ((size_t)2 * mcl + 1 + nci) + mcl + 16);
+  int rc = m->fr_scr.ensure(m, sizeof(int) * ((size_t)2 * mcl + 1 + nci) + mcl + 16);
   if (rc) return rc;
-  int* d_off = (int*)m->fr_scr;
+  int* d_off = (int*)m->fr_scr.p;
   int* d_addr = d_off + mcl + 1;
   int* d_cnt = d_addr + nci;
   uint8_t* d_ch = (uint8_t*)(d_cnt + mcl);

@@ -266,10 +266,9 @@ struct FusionState {
   uint8_t* mark = nullptr;    // per voxel: bit0 hit, bit1 missed this frame (count_hit_/count_miss_ analogue)
   unsigned long long* d_bounds = nullptr;
   int* d_count = nullptr;
-  float* d_pts = nullptr;
-  double* d_ptw = nullptr;
-  int* d_end = nullptr;
-  int cap = 0;
+  DevBuf<float> d_pts;  // per-frame points (or the depth image), grown on demand
+  DevBuf<double> d_ptw;
+  DevBuf<int> d_end;
   double update_min[3] = { 0, 0, 0 }, update_max[3] = { 0, 0, 0 };  // md_->update_min_/max_
   bool reset_updated_box = true;
   double clamp_max_log = 2.1972245773362196;  // logit(p_max = 0.90, algorithm.xml:48) until a frame says otherwise
@@ -321,9 +320,12 @@ double* fusion_logodds_ptr(FuelMap* m, double* clamp_max_log) {
 void fusion_state_destroy(FuelMap* m) {
   FusionState* f = m->fus;
   if (!f) return;
-  void* ptrs[] = { f->logodds, f->rayend, f->mark, f->d_bounds, f->d_count, f->d_pts, f->d_ptw, f->d_end };
+  void* ptrs[] = { f->logodds, f->rayend, f->mark, f->d_bounds, f->d_count };
   for (void* p : ptrs)
     if (p) cudaFree(p);
+  f->d_pts.release();
+  f->d_ptw.release();
+  f->d_end.release();
   delete f;
   m->fus = nullptr;
 }
@@ -373,20 +375,10 @@ static int fusion_frame(FuelMap* m, const float* pts_host, int stride, int n, co
     const int64_t px = ((int64_t)rows * cols + 7) / 8;
     need = px > n ? (int)px : n;
   }
-  if (need > f->cap) {
-    if (f->d_pts) cudaFree(f->d_pts);
-    if (f->d_ptw) cudaFree(f->d_ptw);
-    if (f->d_end) cudaFree(f->d_end);
-    f->d_pts = nullptr;
-    f->d_ptw = nullptr;
-    f->d_end = nullptr;
-    f->cap = 0;
-    const int cap = need + need / 4 + 1024;
-    FUEL_CUDA(m, cudaMalloc(&f->d_pts, sizeof(float) * 4 * cap));  // also holds a uint16 image of <= 8*cap pixels
-    FUEL_CUDA(m, cudaMalloc(&f->d_ptw, sizeof(double) * 3 * cap));
-    FUEL_CUDA(m, cudaMalloc(&f->d_end, sizeof(int) * cap));
-    f->cap = cap;
-  }
+  rc = f->d_pts.ensure(m, 4 * (size_t)need);  // also holds a uint16 image of <= 8 * need pixels
+  if (!rc) rc = f->d_ptw.ensure(m, 3 * (size_t)need);
+  if (!rc) rc = f->d_end.ensure(m, need);
+  if (rc) return rc;
   FusionConsts fc;
   fc.max_ray_length = p->max_ray_length;
   fc.clamp_min = logit(p->p_min);
@@ -400,8 +392,8 @@ static int fusion_frame(FuelMap* m, const float* pts_host, int stride, int n, co
   FUEL_CUDA(m, cudaMemcpyAsync(f->d_bounds, hb, sizeof(hb), cudaMemcpyHostToDevice, s));
   const unsigned nb = (unsigned)((n + 127) / 128);
   if (!cp) {
-    FUEL_CUDA(m, cudaMemcpyAsync(f->d_pts, pts_host, sizeof(float) * ((size_t)stride * (n - 1) + 3), cudaMemcpyHostToDevice, s));
-    classify_points_kernel<<<nb, 128, 0, s>>>(g, fc, f->d_pts, stride, n, cam[0], cam[1], cam[2], f->d_ptw, f->d_end, f->mark,
+    FUEL_CUDA(m, cudaMemcpyAsync(f->d_pts.p, pts_host, sizeof(float) * ((size_t)stride * (n - 1) + 3), cudaMemcpyHostToDevice, s));
+    classify_points_kernel<<<nb, 128, 0, s>>>(g, fc, f->d_pts.p, stride, n, cam[0], cam[1], cam[2], f->d_ptw.p, f->d_end.p, f->mark,
                                               f->rayend, f->d_bounds);
   } else {
     CamConsts cc;
@@ -413,11 +405,11 @@ static int fusion_frame(FuelMap* m, const float* pts_host, int stride, int n, co
     cc.nu = (cols - 2 * cc.margin + cc.skip - 1) / cc.skip;
     cc.nv = (rows - 2 * cc.margin + cc.skip - 1) / cc.skip;
     FUEL_CUDA(m, cudaMemsetAsync(f->d_count, 0, sizeof(int), s));
-    FUEL_CUDA(m, cudaMemcpyAsync(f->d_pts, img_host, sizeof(uint16_t) * (size_t)rows * cols, cudaMemcpyHostToDevice, s));
-    classify_depth_kernel<<<nb, 128, 0, s>>>(g, fc, cc, (const uint16_t*)f->d_pts, cam[0], cam[1], cam[2], f->d_ptw, f->d_end,
+    FUEL_CUDA(m, cudaMemcpyAsync(f->d_pts.p, img_host, sizeof(uint16_t) * (size_t)rows * cols, cudaMemcpyHostToDevice, s));
+    classify_depth_kernel<<<nb, 128, 0, s>>>(g, fc, cc, (const uint16_t*)f->d_pts.p, cam[0], cam[1], cam[2], f->d_ptw.p, f->d_end.p,
                                              f->mark, f->rayend, f->d_bounds, f->d_count);
   }
-  raycast_kernel<<<nb, 128, 0, s>>>(g, f->d_ptw, f->d_end, f->rayend, n, cam[0], cam[1], cam[2], f->mark);
+  raycast_kernel<<<nb, 128, 0, s>>>(g, f->d_ptw.p, f->d_end.p, f->rayend, n, cam[0], cam[1], cam[2], f->mark);
   FUEL_LAUNCHES(m, 2);
   // Every voxel touched this frame lies within max_ray_length of the camera (clipped points, :277-297) and
   // inside the map, so the dense sweep needs no device round trip for its extent.

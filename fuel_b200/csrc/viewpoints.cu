@@ -222,10 +222,10 @@ int sample_viewpoints_impl(FuelMap* m, int ncl, const int32_t* filt_off, const d
   const size_t nd = 2 * (size_t)nc + 3 * (size_t)ncl + 3 * (size_t)(nfilt > 0 ? nfilt : 1) + 7 * n_out;
   const size_t ni = (size_t)ncl + 1 + 3 * n_out;
   const size_t dbytes = (sizeof(double) * nd + 255) & ~(size_t)255;
-  int rc = ensure_fr_scratch(m, dbytes + sizeof(int) * ni);
+  int rc = m->fr_scr.ensure(m, dbytes + sizeof(int) * ni);
   if (rc) return rc;
-  double* d_d = (double*)m->fr_scr;
-  int* d_i = (int*)((uint8_t*)m->fr_scr + dbytes);
+  double* d_d = (double*)m->fr_scr.p;
+  int* d_i = (int*)(m->fr_scr.p + dbytes);
   double *d_off = d_d, *d_avg = d_off + 2 * nc, *d_filt = d_avg + 3 * ncl, *d_pos = d_filt + 3 * (size_t)(nfilt > 0 ? nfilt : 1),
          *d_yaw = d_pos + 3 * n_out, *d_hyaw = d_yaw + n_out;
   int *d_fo = d_i, *d_vis = d_i + ncl + 1, *d_unc = d_vis + n_out, *d_redo = d_unc + n_out;
