@@ -624,8 +624,18 @@ int fuelgpu_frontier_search_begin(FuelMap* m, const double upd_min[3], const dou
 int fuelgpu_frontier_search_end(FuelMap* m, int32_t* n_clusters, int32_t* n_cells, int32_t* n_filtered) {
   if (!m || !n_clusters || !n_cells || !n_filtered) return fuel_fail(m, FUELGPU_EINVAL, "null argument");
   FUEL_CUDA(m, cudaSetDevice(m->dev));
+#ifdef FUEL_PROF
+  const double t0 = prof_now_us();
+#endif
   int rc = frontier_search_end_impl(m, n_clusters, n_cells, n_filtered);
+#ifdef FUEL_PROF
+  const double t1 = prof_now_us();
+  m->end_prof_us[1] = t1 - t0 - m->end_prof_us[0];  // everything of _end but the stream wait
+#endif
   tend(m, T_FRONTIER, frontier_stream_raw(m));
+#ifdef FUEL_PROF
+  m->end_prof_us[2] = prof_now_us() - t1;
+#endif
   return rc;
 }
 

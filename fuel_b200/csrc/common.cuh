@@ -7,6 +7,9 @@
 #include <string.h>
 
 #include <vector>
+#ifdef FUEL_PROF
+#include <chrono>
+#endif
 
 #include "fuelgpu.h"
 
@@ -85,6 +88,9 @@ struct FuelMap {
   DevBuf<uint8_t> tc_buf;  // the other host-facing batch calls (check, evaluate, parameterize, poly, yaw, A*, esdf_sample)
   DevBuf<uint8_t> as_buf;  // A* search scratch (astar.cu)
   size_t as_stride, as_warps;  // layout whose key tables are known empty: per-warp bytes, warps
+#ifdef FUEL_PROF
+  double end_prof_us[3];  // the last fuelgpu_frontier_search_end: stream wait, result assembly, closing event (host µs)
+#endif
 };
 
 extern thread_local char g_fuelgpu_err[512];
@@ -129,6 +135,12 @@ static inline void tend(FuelMap* m, int t, cudaStream_t s = nullptr) {
   m->ev_valid[t] = true;
 }
 #define FUEL_LAUNCHES(m, n) __atomic_fetch_add(&(m)->launches, (long long)(n), __ATOMIC_RELAXED)
+#ifdef FUEL_PROF
+static inline double prof_now_us() {
+  return 1e-3 * (double)std::chrono::duration_cast<std::chrono::nanoseconds>(
+                    std::chrono::steady_clock::now().time_since_epoch()).count();
+}
+#endif
 
 __host__ __device__ static inline int64_t addr_of(const Geom& g, int x, int y, int z) {
   return ((int64_t)x * g.ny + y) * g.nz + z;

@@ -1241,9 +1241,27 @@ __global__ void init_meta_kernel(ClusterMeta* meta, ClusterStat* st, LevelCtl ct
 constexpr int SMALL_CTAS = 8;      // one thread-block cluster (portable maximum)
 constexpr int SMALL_CAP = 32768;   // candidate cells
 constexpr int SMALL_CCAP = 8192;   // clusters (incl. split products)
-// the speculative prefix of the small path's results that comes back with the counters in one copy: a search with more
-// kept cells or clusters fetches the rest with a second, exact-size download
-constexpr int RES_K0 = 12288, RES_C0 = 256;
+// The small path's result block: the kernel's tail writes the arrays fuelgpu_frontier_fetch hands out, in their final
+// order, and the block comes back with the counters in one copy.  A search with more kept cells, clusters or filtered
+// cells than these caps is marshalled on the host from an exact-size download (frontier_marshal).
+constexpr int RES_K0 = 12288, RES_C0 = 256, RES_F0 = 4096;
+constexpr size_t al16(size_t b) { return (b + 15) & ~(size_t)15; }
+// byte offsets in the block: int counters[16] ([0] n_cand [1] R [2] K [3] n_new [4] status [5] C [8] assembled [9] NF),
+// int cell_off[C+1], int filt_off[C+1], double average[3C], int box[6C] (lo xyz, hi xyz), int cell_addr[K],
+// double filtered[3 NF] -- clusters in output order
+constexpr size_t RB_CELL_OFF = 64;
+constexpr size_t RB_FILT_OFF = RB_CELL_OFF + al16(sizeof(int) * (RES_C0 + 1));
+constexpr size_t RB_AVG = RB_FILT_OFF + al16(sizeof(int) * (RES_C0 + 1));
+constexpr size_t RB_BOX = RB_AVG + al16(sizeof(double) * 3 * RES_C0);
+constexpr size_t RB_ADDR = RB_BOX + al16(sizeof(int) * 6 * RES_C0);
+constexpr size_t RB_FILT = RB_ADDR + al16(sizeof(int) * RES_K0);
+constexpr size_t RB_BYTES = RB_FILT + al16(sizeof(double) * 3 * RES_F0);
+// the tail's scratch (ints): per cluster cell count, filtered count, output rank; per kept cell its place in cell_addr
+// and in its cluster's filtered range (kept order); per filtered slot its kept cell, leaf and cluster rank
+constexpr size_t ASM_SCR = 3 * RES_C0 + 2 * RES_K0 + 3 * RES_F0;
+constexpr unsigned TAG_PAD = 0x8000u;  // a kept cell's tag: cluster id | 0x100 if it holds a VoxelGrid centroid
+static_assert(RES_C0 <= 256 && RES_C0 <= SMALL_CTAS * 32, "cluster ids fit a tag byte, one warp per cluster");
+static_assert(RES_K0 % 128 == 0 && sizeof(int) * RES_F0 <= sizeof(unsigned short) * RES_K0, "tail's shared memory");
 
 
 // Small path: the kept/root marks of 32 consecutive cells are one ballot, so the rank scan runs over ceil(n/32) <= 1024
@@ -1325,15 +1343,149 @@ struct SmallBufs {
   ClusterMeta* meta;
   ClusterStat* stat;
   int* counters;  // [0] n_cand (in) [1] R [2] K [3] n_new [4] status [5] C
-  // the result block the host fetches with ONE copy: the eight counters, then the first r_C clusters and r_K kept
-  // cells of meta / stat / k_addr / k_cl / k_leaf / k_cent, laid out as the pinned buffer (result_layout)
-  int* r_counters;
-  ClusterMeta* r_meta;
-  ClusterStat* r_stat;
-  int *r_addr, *r_cl, *r_leaf;
-  float* r_cent;
-  int r_K, r_C;
+  char* res;      // the result block the host fetches with ONE copy (RB_* layout)
+  int* scr;       // ASM_SCR ints for the tail
+  int assemble;   // 0: leave the ordering to the host (counters only)
 };
+
+// ---- the tail of the small path: the result in output order ---------------------------------------------------------
+// The same arrays and order as frontier_build_csr: clusters by (root, path), a cluster's cells in ascending address
+// (= kept index), its filtered cells by (leaf, kept index).  Phase A: cell / filtered counts per cluster (warp-aggregated
+// atomics) and the output rank of every cluster (one warp per cluster, O(C) compares).
+__device__ __forceinline__ void tail_count_item(const int* __restrict__ k_cl, const int* __restrict__ k_leaf,
+                                                int* __restrict__ cnt_cell, int* __restrict__ cnt_filt, int K, int k) {
+  const int c = k < K ? k_cl[k] : -1;
+  const int cf = (k < K && k_leaf[k] >= 0) ? c : -1;
+  const unsigned pc = __match_any_sync(0xffffffffu, c), pf = __match_any_sync(0xffffffffu, cf);
+  const int lane = k & 31;
+  if (c >= 0 && lane == __ffs(pc) - 1) atomicAdd(cnt_cell + c, __popc(pc));
+  if (cf >= 0 && lane == __ffs(pf) - 1) atomicAdd(cnt_filt + cf, __popc(pf));
+}
+__device__ __forceinline__ void tail_rank_warp(const ClusterMeta* __restrict__ meta, int* __restrict__ crank, int C, int c,
+                                               int lane) {
+  const int r0 = meta[c].root;
+  const unsigned p0 = meta[c].path;
+  int lt = 0;
+  for (int c2 = lane; c2 < C; c2 += 32) {
+    const int r2 = meta[c2].root;
+    const unsigned p2 = meta[c2].path;
+    lt += r2 < r0 || (r2 == r0 && (p2 < p0 || (p2 == p0 && c2 < c)));
+  }
+  lt = __reduce_add_sync(0xffffffffu, lt);
+  if (lane == 0) crank[c] = lt;
+}
+// Phase B.  Every CTA first copies the tags of all kept cells into shared memory (tail_tags); then one warp per cluster c
+// writes its CSR offsets (sum of the counts of the clusters ranked before it), average_ and box, and runs once over the
+// tags, four cells per lane, to give each of its cells its place in cell_addr and each of its filtered cells its place
+// in the cluster's filtered range, both in ascending kept index.  Only stores leave the loop.
+__device__ __forceinline__ void tail_tags(const int* __restrict__ k_cl, const int* __restrict__ k_leaf,
+                                          unsigned short* __restrict__ tag, int K) {
+  const int Kp = (K + 127) & ~127;
+  for (int k = threadIdx.x; k < Kp; k += blockDim.x)
+    tag[k] = (unsigned short)(k < K ? (unsigned)k_cl[k] | (k_leaf[k] >= 0 ? 0x100u : 0u) : TAG_PAD);
+}
+__device__ __forceinline__ void tail_place_warp(const ClusterMeta* __restrict__ meta, const ClusterStat* __restrict__ st,
+                                                const unsigned short* __restrict__ tag, int* __restrict__ scr,
+                                                char* __restrict__ res, int K, int C, int c, int lane) {
+  const int *cnt_cell = scr, *cnt_filt = scr + RES_C0, *crank = scr + 2 * RES_C0;
+  int* pos = scr + 3 * RES_C0;
+  int* fpos = pos + RES_K0;
+  const int r = crank[c];
+  int co = 0, fo = 0;
+  for (int c2 = lane; c2 < C; c2 += 32) {
+    if (crank[c2] < r) {
+      co += cnt_cell[c2];
+      fo += cnt_filt[c2];
+    }
+  }
+  co = __reduce_add_sync(0xffffffffu, co);
+  fo = __reduce_add_sync(0xffffffffu, fo);
+  int* cell_off = (int*)(res + RB_CELL_OFF);
+  int* filt_off = (int*)(res + RB_FILT_OFF);
+  if (lane == 0) {
+    cell_off[r] = co;
+    filt_off[r] = fo;
+    if (r == C - 1) {
+      cell_off[C] = co + cnt_cell[c];
+      filt_off[C] = fo + cnt_filt[c];
+    }
+  }
+  if (lane < 3) {
+    ((double*)(res + RB_AVG))[3 * r + lane] = meta[c].mean[lane];
+    ((int*)(res + RB_BOX))[6 * r + lane] = st[c].lo[lane];
+    ((int*)(res + RB_BOX))[6 * r + 3 + lane] = st[c].hi[lane];
+  }
+  const int Kp = (K + 127) & ~127;
+  for (int base = 0; base < Kp; base += 128) {
+    const uint2 w = *(const uint2*)(tag + base + 4 * lane);
+    const unsigned t[4] = { w.x & 0xffffu, w.x >> 16, w.y & 0xffffu, w.y >> 16 };
+    unsigned mine = 0, filt = 0;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if ((t[j] & 0x80ffu) == (unsigned)c) {
+        mine |= 1u << j;
+        if (t[j] & 0x100u) filt |= 1u << j;
+      }
+    }
+    if (!__any_sync(0xffffffffu, mine)) continue;
+    // exclusive prefix over the lanes of (cells, filtered cells), packed 16/16 (at most 128 each)
+    const unsigned v = (unsigned)__popc(mine) | ((unsigned)__popc(filt) << 16);
+    unsigned inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned u = __shfl_up_sync(0xffffffffu, inc, o);
+      if (lane >= o) inc += u;
+    }
+    const unsigned tot = __shfl_sync(0xffffffffu, inc, 31), ex = inc - v;
+    int pm = co + (int)(ex & 0xffffu), pf = fo + (int)(ex >> 16);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if ((mine >> j) & 1u) {
+        pos[base + 4 * lane + j] = pm++;
+        if ((filt >> j) & 1u) fpos[base + 4 * lane + j] = pf++;
+      }
+    }
+    co += (int)(tot & 0xffffu);
+    fo += (int)(tot >> 16);
+  }
+}
+// Phase C, one thread per kept cell: its address to its place; a filtered cell lists (kept index, leaf, cluster rank)
+// in its slot of the filtered range (kept order inside the cluster)
+__device__ __forceinline__ void tail_scatter_item(const int* __restrict__ k_addr, const int* __restrict__ k_cl,
+                                                  const int* __restrict__ k_leaf, const int* __restrict__ scr,
+                                                  int* __restrict__ f_k, int* __restrict__ f_leaf, int* __restrict__ f_r,
+                                                  char* __restrict__ res, int K, int k) {
+  if (k >= K) return;
+  const int *crank = scr + 2 * RES_C0, *pos = scr + 3 * RES_C0, *fpos = pos + RES_K0;
+  ((int*)(res + RB_ADDR))[pos[k]] = k_addr[k];
+  const int lf = k_leaf[k];
+  if (lf >= 0) {
+    const int s = fpos[k];
+    f_k[s] = k;
+    f_leaf[s] = lf;
+    f_r[s] = crank[k_cl[k]];
+  }
+}
+// Phase D, one thread per filtered slot i, the leaves of all slots in shared memory: its place in the cluster is the
+// number of slots of the range with a smaller (leaf, kept index); the centroid goes there as the double fetch returns
+__device__ __forceinline__ void tail_filtered_item(const float* __restrict__ k_cent, const int* __restrict__ f_k,
+                                                   const int* __restrict__ s_leaf, const int* __restrict__ f_r,
+                                                   char* __restrict__ res, int NF, int i) {
+  if (i >= NF) return;
+  const int* filt_off = (const int*)(res + RB_FILT_OFF);
+  const int r = f_r[i], lo = filt_off[r], hi = filt_off[r + 1], lf = s_leaf[i];
+  int pos = lo;
+#pragma unroll 4
+  for (int j = lo; j < hi; ++j) {
+    const int l2 = s_leaf[j];
+    pos += l2 < lf || (l2 == lf && j < i);
+  }
+  const int k = f_k[i];
+  double* out = (double*)(res + RB_FILT);
+  out[3 * pos] = (double)k_cent[3 * k];
+  out[3 * pos + 1] = (double)k_cent[3 * k + 1];
+  out[3 * pos + 2] = (double)k_cent[3 * k + 2];
+}
 
 __global__ void __cluster_dims__(SMALL_CTAS, 1, 1) __launch_bounds__(1024) cluster_small_kernel(Geom g, FParams fp, int8_t* __restrict__ flag,
                                                              int* __restrict__ cellidx, SmallBufs b) {
@@ -1352,11 +1504,12 @@ __global__ void __cluster_dims__(SMALL_CTAS, 1, 1) __launch_bounds__(1024) clust
 #define STAMP() do {} while (0)
 #endif
   STAMP();
+  int* r_counters = (int*)b.res;
   if (n > SMALL_CAP) {
     if (tid == 0) {
       b.counters[4] = 1;
-      b.r_counters[0] = n;
-      b.r_counters[4] = 1;
+      r_counters[0] = n;
+      r_counters[4] = 1;
     }
     return;  // uniform over the whole cluster
   }
@@ -1392,6 +1545,7 @@ __global__ void __cluster_dims__(SMALL_CTAS, 1, 1) __launch_bounds__(1024) clust
       init_meta_item(b.meta, R, c);
       stat_reset_item(b.stat, b.meta, R, c);
     }
+    if (b.assemble) FOR_ITEMS(c, 2 * RES_C0) if (c < 2 * RES_C0) b.scr[c] = 0;  // the tail's per-cluster counts
     cluster.sync();
     STAMP();
     for (int level = 0; level < 40; ++level) {
@@ -1432,33 +1586,43 @@ __global__ void __cluster_dims__(SMALL_CTAS, 1, 1) __launch_bounds__(1024) clust
     }
   }
   FOR_ITEMS(i, n) reset_cellidx_item(b.cell_addr, cellidx, n, i);
-  // the prefix of the results the host reads goes into the result block (every value is final since the last
-  // cluster.sync(), whichever CTA wrote it)
-  if (status == 0 && R > 0 && K > 0) {
-    const int kp = min(K, b.r_K), cp = min(C, b.r_C);
-    FOR_ITEMS(k, kp) {
-      if (k < kp) {
-        b.r_addr[k] = b.k_addr[k];
-        b.r_cl[k] = b.k_cl[k];
-        b.r_leaf[k] = b.k_leaf[k];
-        b.r_cent[3 * k] = b.k_cent[3 * k];
-        b.r_cent[3 * k + 1] = b.k_cent[3 * k + 1];
-        b.r_cent[3 * k + 2] = b.k_cent[3 * k + 2];
-      }
-    }
-    FOR_ITEMS(c, cp) {
-      if (c < cp) {
-        b.r_meta[c] = b.meta[c];
-        b.r_stat[c] = b.stat[c];
-      }
+  // the result in output order (every value the tail reads is final since the last cluster.sync(), whichever CTA
+  // wrote it); the conditions are uniform over the cluster
+  int assembled = 0, NF = 0;
+  if (b.assemble && status == 0 && R > 0 && K > 0 && K <= RES_K0 && C <= RES_C0) {
+    __shared__ __align__(16) unsigned short s_tag[RES_K0];  // phase B: kept-cell tags; phase D: the slots' leaves
+    int* f_k = b.scr + 3 * RES_C0 + 2 * RES_K0;
+    int* f_leaf = f_k + RES_F0;
+    int* f_r = f_leaf + RES_F0;
+    const int gw = tid >> 5, lane = tid & 31;  // one warp per cluster: 8 x 32 warps >= RES_C0
+    FOR_ITEMS(k, K) tail_count_item(b.k_cl, b.k_leaf, b.scr, b.scr + RES_C0, K, k);
+    if (gw < C) tail_rank_warp(b.meta, b.scr + 2 * RES_C0, C, gw, lane);
+    cluster.sync();
+    STAMP();
+    tail_tags(b.k_cl, b.k_leaf, s_tag, K);
+    __syncthreads();
+    if (gw < C) tail_place_warp(b.meta, b.stat, s_tag, b.scr, b.res, K, C, gw, lane);
+    cluster.sync();
+    STAMP();
+    NF = ((const int*)(b.res + RB_FILT_OFF))[C];
+    if (NF <= RES_F0) {  // (uniform)
+      FOR_ITEMS(k, K) tail_scatter_item(b.k_addr, b.k_cl, b.k_leaf, b.scr, f_k, f_leaf, f_r, b.res, K, k);
+      cluster.sync();
+      STAMP();
+      int* s_leaf = (int*)s_tag;  // (RES_F0 ints fit in the tags' space)
+      for (int i = threadIdx.x; i < NF; i += blockDim.x) s_leaf[i] = f_leaf[i];
+      __syncthreads();
+      FOR_ITEMS(i, NF) tail_filtered_item(b.k_cent, f_k, s_leaf, f_r, b.res, NF, i);
+      STAMP();
+      assembled = 1;
     }
   }
   if (tid == 0) {
     b.counters[4] = status;
     b.counters[5] = C;
-    const int out[8] = { n, R, K, b.counters[3], status, C, b.counters[6], b.counters[7] };
+    const int out[10] = { n, R, K, b.counters[3], status, C, b.counters[6], b.counters[7], assembled, NF };
 #pragma unroll
-    for (int j = 0; j < 8; ++j) b.r_counters[j] = out[j];
+    for (int j = 0; j < 10; ++j) r_counters[j] = out[j];
   }
 #undef FOR_ITEMS
 }
@@ -1513,20 +1677,24 @@ struct FrontierState {
   DevBuf<float> k_cent;
   DevBuf<ClusterStat> stat;
   DevBuf<ClusterMeta> meta;
-  DevBuf<char> res;  // the small path's result block (SmallBufs::r_*), fetched with one copy
-  bool small_ready = false;
+  DevBuf<char> res;     // the small path's result block (RB_* layout), fetched with one copy
+  DevBuf<int> asm_scr;  // scratch of the kernel's tail (ASM_SCR)
   // a search that has been enqueued (begin) but not yet collected (end)
   bool pend_active = false, pend_empty = true;
   FParams pend_fp;
   SweepPlan pend_plan;
-  HostView pend_hv;
   cudaStream_t stream = nullptr;  // the frontier subsystem's own stream
   cudaEvent_t ev_in = nullptr;
   cudaEvent_t ev_out = nullptr;  // end of the last enqueued search: writers of `occ` on the main stream wait for it
   bool ev_out_valid = false;
-  DevBuf<char, true> h_pin;  // pinned host staging for the result download
+  DevBuf<char, true> h_pin;  // pinned host staging for the exact-size download (frontier_marshal)
+  // pinned copies of the result block, used in turn: a search fills the one that does not hold the result of the last
+  // collected search, so fuelgpu_frontier_fetch may still read that one after the next search_begin
+  DevBuf<char, true> h_res[2];
+  int pend_blk = 0;  // block the pending search is copied into
+  int res_blk = -1;  // block holding the result of the last collected search; -1: the h_* vectors hold it
   int* d_counters = nullptr;  // [0] n_cand [1] n_roots [2] n_kept [3] n_new [4] small-path status [5] C
-  // results of the last search (host side, CSR)
+  // results of the last search marshalled on the host (CSR)
   std::vector<int32_t> h_cell_off, h_cell_addr, h_filt_off;
   std::vector<double> h_filtered, h_avg, h_bmin, h_bmax;
   int cell_order = FUELGPU_CELLS_BY_ADDRESS;  // fuelgpu_frontier_set_cell_order
@@ -1583,6 +1751,7 @@ void frontier_state_destroy(FuelMap* m) {
   f->seed.release(); f->is_root.release(); f->is_kept.release(); f->root_rank.release();
   f->kept_off.release(); f->cell_cls.release(); f->k_addr.release(); f->k_cl.release();
   f->k_leaf.release(); f->k_cent.release(); f->stat.release(); f->meta.release(); f->res.release();
+  f->asm_scr.release(); f->h_res[0].release(); f->h_res[1].release();
   delete f;
   m->fs = nullptr;
 }
@@ -1985,6 +2154,7 @@ static void frontier_make_params(FuelMap* m, const double umin[3], const double 
   *out = fp;
 }
 
+// the result of the last collected search becomes empty (fuelgpu_frontier_fetch returns nothing)
 static void frontier_clear_results(FrontierState* f) {
   f->h_cell_off.assign(1, 0);
   f->h_cell_addr.clear();
@@ -1993,8 +2163,14 @@ static void frontier_clear_results(FrontierState* f) {
   f->h_avg.clear();
   f->h_bmin.clear();
   f->h_bmax.clear();
-  f->pend_active = false;
-  f->pend_empty = true;
+  f->res_blk = -1;
+}
+
+// FUELGPU_FRONTIER_HOST_CSR=1 (read by every search_begin): the small path returns its raw arrays and the host orders
+// them (frontier_build_csr), as the large path does -- the reference the device-built result is tested against
+static bool frontier_host_csr() {
+  const char* e = getenv("FUELGPU_FRONTIER_HOST_CSR");
+  return e && *e && strcmp(e, "0") != 0;
 }
 
 int frontier_search_begin_impl(FuelMap* m, const double umin[3], const double umax[3],
@@ -2005,13 +2181,7 @@ int frontier_search_begin_impl(FuelMap* m, const double umin[3], const double um
   FParams fp;
   frontier_make_params(m, umin, umax, p, &fp);
 
-  f->h_cell_off.assign(1, 0);
-  f->h_cell_addr.clear();
-  f->h_filt_off.assign(1, 0);
-  f->h_filtered.clear();
-  f->h_avg.clear();
-  f->h_bmin.clear();
-  f->h_bmax.clear();
+  // (the result of the last collected search stays readable until the next search_end)
   f->pend_active = false;
   f->pend_empty = true;
 
@@ -2022,7 +2192,7 @@ int frontier_search_begin_impl(FuelMap* m, const double umin[3], const double um
     const int rc = sweep_classify(m, fp, pl, s);
     if (rc) return rc;
   }
-  // ---- small path: one compaction + ONE single-CTA launch, one host sync ------------------------
+  // ---- small path: one compaction + ONE cluster launch, one result copy, one host sync --------------------------
   {
     ENSURE(f->cell_addr, SMALL_CAP); ENSURE(f->cell_cls, SMALL_CAP); ENSURE(f->parent, SMALL_CAP);
     ENSURE(f->claim, SMALL_CAP); ENSURE(f->csize, SMALL_CAP); ENSURE(f->seed, SMALL_CAP);
@@ -2030,10 +2200,11 @@ int frontier_search_begin_impl(FuelMap* m, const double umin[3], const double um
     ENSURE(f->kept_off, SMALL_CAP); ENSURE(f->k_addr, SMALL_CAP); ENSURE(f->k_cl, SMALL_CAP);
     ENSURE(f->k_leaf, SMALL_CAP); ENSURE(f->k_cent, (size_t)3 * SMALL_CAP);
     ENSURE(f->meta, SMALL_CCAP); ENSURE(f->stat, SMALL_CCAP);
-    // one host sync and ONE copy in the common case: the kernel writes the counters and a speculative prefix of the
-    // results (RES_K0 cells, RES_C0 clusters) into one block; a second download only if they did not fit
-    const ResultLayout rl = result_layout(RES_K0, RES_C0);
-    ENSURE(f->res, 64 + rl.bytes);
+    ENSURE(f->res, RB_BYTES); ENSURE(f->asm_scr, ASM_SCR);
+    // the BFS cell order re-derives the cells' order on the host from the marshalled arrays
+    const bool assemble = !frontier_host_csr() && f->cell_order != FUELGPU_CELLS_BFS;
+    const int blk = f->res_blk == 0 ? 1 : 0;
+    ENSURE(f->h_res[blk], RB_BYTES);  // (a fixed size: allocated once, never replaced)
     sweep_compact(m, fp, pl, f->cellidx, SMALL_CAP, s);
     SmallBufs sb;
     sb.cell_addr = f->cell_addr.p; sb.parent = f->parent.p; sb.claim = f->claim.p; sb.csize = f->csize.p;
@@ -2041,20 +2212,13 @@ int frontier_search_begin_impl(FuelMap* m, const double umin[3], const double um
     sb.kept_off = f->kept_off.p; sb.cell_cls = f->cell_cls.p; sb.k_addr = f->k_addr.p; sb.k_cl = f->k_cl.p;
     sb.k_leaf = f->k_leaf.p; sb.k_cent = f->k_cent.p; sb.meta = f->meta.p; sb.stat = f->stat.p;
     sb.counters = f->d_counters;
-    {
-      char* rb = f->res.p + 64;
-      sb.r_counters = (int*)f->res.p;
-      sb.r_meta = (ClusterMeta*)(rb + rl.meta); sb.r_stat = (ClusterStat*)(rb + rl.stat);
-      sb.r_addr = (int*)(rb + rl.addr); sb.r_cl = (int*)(rb + rl.cl); sb.r_leaf = (int*)(rb + rl.leaf);
-      sb.r_cent = (float*)(rb + rl.cent);
-      sb.r_K = RES_K0;
-      sb.r_C = RES_C0;
-    }
+    sb.res = f->res.p;
+    sb.scr = f->asm_scr.p;
+    sb.assemble = assemble ? 1 : 0;
     cluster_small_kernel<<<SMALL_CTAS, 1024, 0, s>>>(g, fp, m->flag, f->cellidx, sb);
     FUEL_LAUNCHES(m, 1);
-    ENSURE(f->h_pin, 64 + rl.bytes);
-    FUEL_CUDA(m, cudaMemcpyAsync(f->h_pin.p, f->res.p, 64 + rl.bytes, cudaMemcpyDeviceToHost, s));
-    result_view(rl, f->h_pin.p + 64, &f->pend_hv);
+    FUEL_CUDA(m, cudaMemcpyAsync(f->h_res[blk].p, f->res.p, assemble ? RB_BYTES : RB_CELL_OFF, cudaMemcpyDeviceToHost, s));
+    f->pend_blk = blk;
     f->pend_fp = fp;
     f->pend_plan = pl;
     f->pend_active = true;
@@ -2071,6 +2235,10 @@ int frontier_search_end_impl(FuelMap* m, int32_t* n_clusters, int32_t* n_cells, 
   const Geom& g = m->g;
   cudaStream_t s = m->fs->stream;
   *n_clusters = *n_cells = *n_filtered = 0;
+  frontier_clear_results(f);
+#ifdef FUEL_PROF
+  m->end_prof_us[0] = 0.0;
+#endif
   if (f->pend_empty || !f->pend_active) {
     f->pend_active = false;
     return 0;
@@ -2080,15 +2248,26 @@ int frontier_search_end_impl(FuelMap* m, int32_t* n_clusters, int32_t* n_cells, 
   const SweepPlan pl = f->pend_plan;
   int n_cand = 0;
   {
-    const int* cnt = (const int*)f->h_pin.p;
-    HostView& hv = f->pend_hv;
+    const int* cnt = (const int*)f->h_res[f->pend_blk].p;
+#ifdef FUEL_PROF
+    const double t0 = prof_now_us();
+#endif
     FUEL_CUDA(m, cudaStreamSynchronize(s));
+#ifdef FUEL_PROF
+    m->end_prof_us[0] = prof_now_us() - t0;
+#endif
     n_cand = cnt[0];
     if (n_cand == 0) return 0;
     if (cnt[4] == 0) {
       const int R = cnt[1], K = cnt[2], C = cnt[5];
       if (R == 0 || K == 0) return 0;
-      if (K <= RES_K0 && C <= RES_C0) return frontier_build_csr(m, K, C, hv, n_clusters, n_cells, n_filtered);
+      if (cnt[8]) {  // ordered on the device: the block is the result
+        *n_clusters = C;
+        *n_cells = K;
+        *n_filtered = cnt[9];
+        f->res_blk = f->pend_blk;
+        return 0;
+      }
       return frontier_marshal(m, K, C, n_clusters, n_cells, n_filtered);
     }
     // capacity exceeded (status 1: cells, 2: clusters): fall through to the multi-kernel path.
@@ -2250,6 +2429,8 @@ int frontier_search_from_candidates_impl(FuelMap* m, const double umin[3], const
   FParams fp;
   frontier_make_params(m, umin, umax, p, &fp);
   frontier_clear_results(f);
+  f->pend_active = false;
+  f->pend_empty = true;
   *n_clusters = *n_cells = *n_filtered = 0;
   if (n <= 0) return 0;
   for (int i = 1; i < n; ++i)
@@ -2279,6 +2460,24 @@ int frontier_search_impl(FuelMap* m, const double umin[3], const double umax[3],
 int frontier_fetch_impl(FuelMap* m, int32_t* cell_offsets, int32_t* cell_addr, int32_t* filt_offsets,
                         double* filtered, double* average, double* box_min, double* box_max) {
   FrontierState* f = m->fs;
+  if (f->res_blk >= 0) {  // the block the small path's kernel ordered
+    const char* rb = f->h_res[f->res_blk].p;
+    const int* cnt = (const int*)rb;
+    const int K = cnt[2], C = cnt[5], NF = cnt[9];
+    const Geom& g = m->g;
+    if (cell_offsets) memcpy(cell_offsets, rb + RB_CELL_OFF, sizeof(int32_t) * (C + 1));
+    if (cell_addr) memcpy(cell_addr, rb + RB_ADDR, sizeof(int32_t) * K);
+    if (filt_offsets) memcpy(filt_offsets, rb + RB_FILT_OFF, sizeof(int32_t) * (C + 1));
+    if (filtered) memcpy(filtered, rb + RB_FILT, sizeof(double) * 3 * NF);
+    if (average) memcpy(average, rb + RB_AVG, sizeof(double) * 3 * C);
+    const int* box = (const int*)(rb + RB_BOX);
+    for (int r = 0; r < C; ++r)
+      for (int a = 0; a < 3; ++a) {  // (the expression of frontier_build_csr)
+        if (box_min) box_min[3 * r + a] = (box[6 * r + a] + 0.5) * g.res + g.origin[a];
+        if (box_max) box_max[3 * r + a] = (box[6 * r + 3 + a] + 0.5) * g.res + g.origin[a];
+      }
+    return 0;
+  }
   if (cell_offsets) memcpy(cell_offsets, f->h_cell_off.data(), sizeof(int32_t) * f->h_cell_off.size());
   if (cell_addr) memcpy(cell_addr, f->h_cell_addr.data(), sizeof(int32_t) * f->h_cell_addr.size());
   if (filt_offsets) memcpy(filt_offsets, f->h_filt_off.data(), sizeof(int32_t) * f->h_filt_off.size());
@@ -2316,6 +2515,12 @@ int frontier_is_changed_impl(FuelMap* m, int32_t mcl, const int32_t* offs, const
 extern "C" __attribute__((visibility("default"))) int fuelgpu_debug_frontier_prof(FuelMap* m, long long* out,
                                                                                   int n) {
   cudaMemcpy(out, (long long*)(m->fs->d_counters + 8), sizeof(long long) * n, cudaMemcpyDeviceToHost);
+  return 0;
+}
+// debug-only: host µs of the last fuelgpu_frontier_search_end, split into the wait for the frontier stream, the
+// result assembly and the closing timing event
+extern "C" __attribute__((visibility("default"))) int fuelgpu_debug_frontier_end_prof(FuelMap* m, double* out) {
+  for (int i = 0; i < 3; ++i) out[i] = m->end_prof_us[i];
   return 0;
 }
 #endif

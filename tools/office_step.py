@@ -5,9 +5,13 @@ Prints, for one `replan_resident` each:
   * the device timeline of the overlapped step (`overlap=True`, as the metric runs it): every kernel, copy and memset
     on every stream, start and end in microseconds after the first device activity of the step (torch.profiler);
   * the same kernels with the stages back to back (`overlap=False`);
-  * the host time of `fuelgpu_frontier_search_end` (the wait for the frontier stream plus the result marshalling) and
-    of `FrontierFinder._fetch`, and of the whole `search_box_end`;
+  * the host time of `fuelgpu_frontier_search_end` (the wait for the frontier stream plus the result hand-off) and
+    of `FrontierFinder._fetch`, and of the whole `search_box_end`; in a FUEL_PROF build, `search_end` with the device
+    idle split into the stream wait, the rest of `_end` (the host marshalling when the host orders the result) and
+    the closing timing event;
   * in a FUEL_PROF build, the %globaltimer stamps of `cluster_small_kernel` (one per cluster.sync()), by phase.
+
+FUELGPU_FRONTIER_HOST_CSR=1 times the host-ordered result instead of the device-ordered one.
 
   python tools/office_step.py [--reps 20] [--trace DIR]
 """
@@ -107,7 +111,11 @@ def host_times(P, reps):
     print("fuelgpu_frontier_search_end %.1f us (wait for the frontier stream + marshalling), FrontierFinder._fetch %.1f us, "
           "together %.1f us; step %.1f us" % (med(t_end), med(t_fetch), med(t_all), 1e3 * float(np.median(t_step))))
     # the marshalling alone: the same calls once the frontier stream is known to be idle
-    t_m, t_f = [], []
+    so = C.CDLL(P.fuel._lib.SO)
+    split = hasattr(so, "fuelgpu_debug_frontier_end_prof")
+    if split:
+        so.fuelgpu_debug_frontier_end_prof.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
+    t_m, t_f, parts = [], [], []
     for _ in range(reps):
         P.l2_flush()
         P._frontier_begin()
@@ -119,8 +127,18 @@ def host_times(P, reps):
         c = time.perf_counter()
         t_m.append(b - a)
         t_f.append(c - b)
+        if split:
+            buf = (C.c_double * 3)()
+            so.fuelgpu_debug_frontier_end_prof(h, buf)
+            parts.append(list(buf))
     print("with the device idle: fuelgpu_frontier_search_end %.1f us, _fetch %.1f us (%d clusters, %d cells, %d filtered)"
           % (med(t_m), med(t_f), nc.value, ncell.value, nf.value))
+    if split:
+        p = np.median(np.array(parts), axis=0)
+        print("  search_end split (FUEL_PROF steady clock, median): cudaStreamSynchronize %.1f us, result assembly %.1f us, "
+              "tend %.1f us, rest (ABI entry, ctypes) %.1f us" % (p[0], p[1], p[2], med(t_m) - p.sum()))
+    else:
+        print("  (search_end split into stream wait / result assembly / tend: FUEL_PROF builds only)")
 
 
 def prof_stamps(P):
@@ -140,9 +158,13 @@ def prof_stamps(P):
     head = ["init_parent", "union", "flatten", "claim", "assign", "mark", "chunk_scan", "gather+init_meta"]
     level = ["stat_accum", "mean+downsample", "cov", "pca", "side_count", "split_alloc", "relabel", "next_level"]
     names = list(head)
-    while len(names) < len(t) - 1:
+    # the last level stops after its relabel (no next_level stamp); a search whose result the kernel ordered ends with
+    # the four phases of its tail
+    tail = ["tail count+rank", "tail places", "tail scatter", "tail filtered"] if (len(t) - 1 - len(head)) % len(level) == 3 else []
+    while len(names) < len(t) - 1 - len(tail):
         lv = (len(names) - len(head)) // len(level)
         names += ["L%d %s" % (lv, n) for n in level]
+    names += tail
     d = np.diff(t) / 1e3
     print("== cluster_small_kernel: %d stamps, %.1f us from the first to the last ==" % (len(t), (t[-1] - t[0]) / 1e3))
     for n, v in zip(names, d):
