@@ -11,6 +11,7 @@ from .bspline_optimizer import BsplineOptimizer  # noqa: F401
 from .frontier_finder import Frontier, FrontierFinder  # noqa: F401
 from .non_uniform_bspline import NonUniformBspline  # noqa: F401
 from .sdf_map import EDTEnvironment, SDFMap  # noqa: F401
+from .view_node import ViewNode  # noqa: F401
 
-__all__ = ["SDFMap", "EDTEnvironment", "FrontierFinder", "Frontier", "BsplineOptimizer", "NonUniformBspline",
+__all__ = ["SDFMap", "EDTEnvironment", "FrontierFinder", "Frontier", "BsplineOptimizer", "NonUniformBspline", "ViewNode",
            "FuelGpuError", "lib"]

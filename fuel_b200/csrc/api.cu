@@ -274,6 +274,7 @@ int fuelgpu_map_destroy(FuelMap* m) {
   m->fr_scr.release();
   m->tc_buf.release();
   m->as_buf.release();
+  m->vc_buf.release();
   for (int t = 0; t < T_COUNT; ++t) {
     if (m->ev0[t]) cudaEventDestroy(m->ev0[t]);
     if (m->ev1[t]) cudaEventDestroy(m->ev1[t]);
@@ -1241,11 +1242,7 @@ int fuelgpu_yaw_explore_batch(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar
   return st.download();
 }
 
-static int check_astar_args(FuelMap* m, int32_t B, const void* start, const void* goal, const FuelAstarParams* p,
-                            const void* info, int32_t path_max, const void* path, int32_t w_max, const void* n_wp,
-                            const void* waypts) {
-  if (!m) return fuel_fail(nullptr, FUELGPU_EINVAL, "null map");
-  if (B < 0) return fuel_fail(m, FUELGPU_EINVAL, "negative batch");
+static int check_astar_params(FuelMap* m, const FuelAstarParams* p) {
   if (!p) return fuel_fail(m, FUELGPU_EINVAL, "null params");
   // above 1e-3 the reference's neighbour loop (astar2.cpp:90-94) makes exactly the 26 steps
   if (!(p->resolution > 1e-3 && p->resolution <= 1.7976931348623157e308))
@@ -1254,6 +1251,16 @@ static int check_astar_args(FuelMap* m, int32_t B, const void* start, const void
   if (p->allocate_num < 2 || p->max_iter < 1)
     return fuel_fail(m, FUELGPU_EINVAL, "allocate_num must be at least 2 and max_iter at least 1");
   if (p->allocate_num > (1 << 28)) return fuel_fail(m, FUELGPU_EINVAL, "allocate_num above 2^28");
+  return 0;
+}
+
+static int check_astar_args(FuelMap* m, int32_t B, const void* start, const void* goal, const FuelAstarParams* p,
+                            const void* info, int32_t path_max, const void* path, int32_t w_max, const void* n_wp,
+                            const void* waypts) {
+  if (!m) return fuel_fail(nullptr, FUELGPU_EINVAL, "null map");
+  if (B < 0) return fuel_fail(m, FUELGPU_EINVAL, "negative batch");
+  const int rc = check_astar_params(m, p);
+  if (rc) return rc;
   if (w_max < 3) return fuel_fail(m, FUELGPU_EINVAL, "w_max must be at least 3");
   if (path && path_max < 1) return fuel_fail(m, FUELGPU_EINVAL, "path_max must be at least 1 with a path buffer");
   if (B > 0 && (!start || !goal || !info || !n_wp || !waypts)) return fuel_fail(m, FUELGPU_EINVAL, "null argument");
@@ -1291,6 +1298,52 @@ int fuelgpu_astar_batch(FuelMap* m, int32_t B, const double* start, const double
   rc = st.upload();
   if (rc) return rc;
   rc = astar_impl(m, B, d_s, d_g, p, d_info, path_max, d_path, w_max, d_n, d_wp);
+  if (rc) return rc;
+  return st.download();
+}
+
+static int check_view_cost_args(FuelMap* m, int32_t P, const void* p1, const void* p2, const void* y1, const void* y2,
+                                const void* v1, const FuelViewCostParams* p, const void* info, int32_t path_max,
+                                const void* path) {
+  if (!m) return fuel_fail(nullptr, FUELGPU_EINVAL, "null map");
+  if (P < 0) return fuel_fail(m, FUELGPU_EINVAL, "negative batch");
+  if (!p) return fuel_fail(m, FUELGPU_EINVAL, "null params");
+  if (!finite_pos(p->vm) || !finite_pos(p->yd)) return fuel_fail(m, FUELGPU_EINVAL, "vm and yd must be finite and positive");
+  if (!isfinite(p->w_dir)) return fuel_fail(m, FUELGPU_EINVAL, "w_dir must be finite");
+  const int rc = check_astar_params(m, &p->astar);
+  if (rc) return rc;
+  if (path && path_max < 1) return fuel_fail(m, FUELGPU_EINVAL, "path_max must be at least 1 with a path buffer");
+  if (P > 0 && (!p1 || !p2 || !y1 || !y2 || !v1 || !info)) return fuel_fail(m, FUELGPU_EINVAL, "null argument");
+  return 0;
+}
+
+int fuelgpu_view_cost_batch_dev(FuelMap* m, int32_t P, const void* p1_dev, const void* p2_dev, const void* y1_dev,
+                                const void* y2_dev, const void* v1_dev, const FuelViewCostParams* p, void* info_dev,
+                                int32_t path_max, void* path_dev) {
+  int rc = check_view_cost_args(m, P, p1_dev, p2_dev, y1_dev, y2_dev, v1_dev, p, info_dev, path_max, path_dev);
+  if (rc) return rc;
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  return view_cost_impl(m, P, (const double*)p1_dev, (const double*)p2_dev, (const double*)y1_dev,
+                        (const double*)y2_dev, (const double*)v1_dev, p, (FuelViewCostInfo*)info_dev, path_max,
+                        (double*)path_dev);
+}
+
+int fuelgpu_view_cost_batch(FuelMap* m, int32_t P, const double* p1, const double* p2, const double* y1,
+                            const double* y2, const double* v1, const FuelViewCostParams* p, FuelViewCostInfo* info,
+                            int32_t path_max, double* path) {
+  int rc = check_view_cost_args(m, P, p1, p2, y1, y2, v1, p, info, path_max, path);
+  if (rc) return rc;
+  if (P == 0) return 0;
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  const size_t np = (size_t)P;
+  double *d_p1, *d_p2, *d_y1, *d_y2, *d_v1, *d_path;
+  FuelViewCostInfo* d_info;
+  HostStaging st(m);
+  st.in(&d_p1, p1, np * 3).in(&d_p2, p2, np * 3).in(&d_y1, y1, np).in(&d_y2, y2, np).in(&d_v1, v1, np * 3);
+  st.out(&d_info, info, np).out(&d_path, path, np * path_max * 3);
+  rc = st.upload();
+  if (rc) return rc;
+  rc = view_cost_impl(m, P, d_p1, d_p2, d_y1, d_y2, d_v1, p, d_info, path_max, d_path);
   if (rc) return rc;
   return st.download();
 }

@@ -133,11 +133,16 @@ struct NbrShared {  // one warp's 26 neighbour results, written in parallel and 
   FuelPathInfo inf;  // lane 0: the result of the current search
 };
 
+// kRaw: the search of ViewNode::searchPath (active_perception/src/graph_node.cpp:48-57) over the pairs whose straight
+// line is blocked.  The queries are list[0 .. *n_list) of the pair arrays, a count the line test leaves on the device,
+// and each writes getPath() with its Astar::pathLength (astar2.cpp:169-175) into info.length: no shortenPath, branch
+// or tour.
+template <bool kRaw>
 __global__ void __launch_bounds__(AS_THREADS)
 astar_kernel(Geom g, const uint8_t* __restrict__ occ, AsConsts c, int B, const double* __restrict__ start,
              const double* __restrict__ goal, uint8_t* __restrict__ scratch, int* __restrict__ counter,
              FuelPathInfo* __restrict__ info_out, double* __restrict__ path_out, int32_t* __restrict__ nwp_out,
-             double* __restrict__ wp_out) {
+             double* __restrict__ wp_out, const int* __restrict__ n_list, const int* __restrict__ list) {
   __shared__ NbrShared sh_all[AS_WARPS];
   const int lane = threadIdx.x & 31, wl = threadIdx.x >> 5;
   NbrShared& sh = sh_all[wl];
@@ -167,7 +172,8 @@ astar_kernel(Geom g, const uint8_t* __restrict__ occ, AsConsts c, int B, const d
     int b = 0;
     if (lane == 0) b = atomicAdd(counter, 1);
     b = __shfl_sync(0xffffffffu, b, 0);
-    if (b >= B) return;
+    if (b >= (kRaw ? *n_list : B)) return;
+    if (kRaw) b = list[b];
     const double sp[3] = { start[3 * b], start[3 * b + 1], start[3 * b + 2] };
     const double ep[3] = { goal[3 * b], goal[3 * b + 1], goal[3 * b + 2] };
     FuelPathInfo& inf = sh.inf;
@@ -348,6 +354,20 @@ astar_kernel(Geom g, const uint8_t* __restrict__ occ, AsConsts c, int B, const d
       for (int i = lane; i < c.path_max * 3; i += 32) dst[i] = i < 3 * ncopy ? ps[i] : 0.0;
     }
     __syncwarp();
+    if (kRaw) {
+      if (lane == 0) {
+        if (end_node >= 0) {
+          double len = 0.0;  // Astar::pathLength(getPath())
+          for (int k = 0; k + 1 < n_path; ++k)
+            len += norm3(ps[3 * k + 3] - ps[3 * k], ps[3 * k + 4] - ps[3 * k + 1], ps[3 * k + 5] - ps[3 * k + 2]);
+          inf.length = len;
+        }
+        info_out[b] = inf;
+      }
+      for (int i = lane; i < n_ins; i += 32) tab[slot[i]].w = -1;
+      __syncwarp();
+      continue;
+    }
     if (lane == 0 && end_node >= 0) {
       // shortenPath (:295-325), in place: the short tour never outgrows the path read so far
       const double last[3] = { ps[3 * (n_path - 1)], ps[3 * (n_path - 1) + 1], ps[3 * (n_path - 1) + 2] };
@@ -447,8 +467,10 @@ static void astar_layout(int A, AsConsts* c) {
 
 constexpr size_t AS_BUDGET = (size_t)4 << 30;  // bytes of search scratch the warps running at once may use
 
-int astar_impl(FuelMap* m, int B, const double* start_dev, const double* goal_dev, const FuelAstarParams* p,
-               FuelPathInfo* info_dev, int path_max, double* path_dev, int w_max, int32_t* nwp_dev, double* wp_dev) {
+// One launch of astar_kernel<raw> over a pool of `alloc` nodes per search.
+static int astar_launch(FuelMap* m, bool raw, int B, const int* n_list, const int* list, const double* start_dev,
+                        const double* goal_dev, const FuelAstarParams* p, int alloc, FuelPathInfo* info_dev, int path_max,
+                        double* path_dev, int w_max, int32_t* nwp_dev, double* wp_dev) {
   if (B == 0) return 0;
   AsConsts c;
   memset(&c, 0, sizeof(c));
@@ -456,11 +478,11 @@ int astar_impl(FuelMap* m, int B, const double* start_dev, const double* goal_de
   c.inv_res = 1.0 / p->resolution;  // Astar::setResolution / init (:28, :44)
   c.lambda = p->lambda_heu;
   c.tie = 1.0 + 1.0 / 1000;  // tie_breaker_ (:23)
-  c.alloc = p->allocate_num;
+  c.alloc = alloc;
   c.max_iter = p->max_iter;
   c.w_max = w_max;
   c.path_max = path_dev ? path_max : 0;
-  astar_layout(p->allocate_num, &c);
+  astar_layout(alloc, &c);
   size_t W = (size_t)B;
   W = std::min(W, (size_t)m->sm_count * 32);
   W = std::min(W, std::max((size_t)1, AS_BUDGET / c.stride));
@@ -481,9 +503,32 @@ int astar_impl(FuelMap* m, int B, const double* start_dev, const double* goal_de
   }
   int* counter = (int*)m->as_buf.p;
   FUEL_CUDA(m, cudaMemsetAsync(counter, 0, sizeof(int), m->stream));
-  astar_kernel<<<(unsigned)blocks, AS_THREADS, 0, m->stream>>>(m->g, m->occ, c, B, start_dev, goal_dev, scr, counter,
-                                                              info_dev, path_dev, nwp_dev, wp_dev);
+  if (raw)
+    astar_kernel<true><<<(unsigned)blocks, AS_THREADS, 0, m->stream>>>(m->g, m->occ, c, B, start_dev, goal_dev, scr,
+                                                                       counter, info_dev, path_dev, nullptr, nullptr,
+                                                                       n_list, list);
+  else
+    astar_kernel<false><<<(unsigned)blocks, AS_THREADS, 0, m->stream>>>(m->g, m->occ, c, B, start_dev, goal_dev, scr,
+                                                                        counter, info_dev, path_dev, nwp_dev, wp_dev,
+                                                                        nullptr, nullptr);
   FUEL_LAUNCHES(m, 1);
   FUEL_CUDA(m, cudaGetLastError());
   return 0;
+}
+
+int astar_impl(FuelMap* m, int B, const double* start_dev, const double* goal_dev, const FuelAstarParams* p,
+               FuelPathInfo* info_dev, int path_max, double* path_dev, int w_max, int32_t* nwp_dev, double* wp_dev) {
+  return astar_launch(m, false, B, nullptr, nullptr, start_dev, goal_dev, p, p->allocate_num, info_dev, path_max,
+                      path_dev, w_max, nwp_dev, wp_dev);
+}
+
+int astar_raw_impl(FuelMap* m, int P, const int* n_list_dev, const int* list_dev, const double* p1_dev,
+                   const double* p2_dev, const FuelAstarParams* p, FuelPathInfo* info_dev, int path_max,
+                   double* path_dev) {
+  // A search expands at most max_iter nodes and each expansion allocates and pushes at most 26, so it never holds more
+  // than 1 + 26 * max_iter nodes or open-set entries: a pool of min(allocate_num, 26 * max_iter + 2) ends every search
+  // where allocate_num does, and keeps the per-warp scratch small at the reference's allocate_num of 1 000 000.
+  const int alloc = (int)std::min<long long>(p->allocate_num, 26LL * p->max_iter + 2);
+  return astar_launch(m, true, P, n_list_dev, list_dev, p1_dev, p2_dev, p, alloc, info_dev, path_max, path_dev, 0,
+                      nullptr, nullptr);
 }

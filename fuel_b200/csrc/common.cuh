@@ -87,6 +87,7 @@ struct FuelMap {
   char err[512];
   DevBuf<uint8_t> tc_buf;  // the other host-facing batch calls (check, evaluate, parameterize, poly, yaw, A*, esdf_sample)
   DevBuf<uint8_t> as_buf;  // A* search scratch (astar.cu)
+  DevBuf<uint8_t> vc_buf;  // view cost: the blocked-line list and the searches' results (view_cost.cu)
   size_t as_stride, as_warps;  // layout whose key tables are known empty: per-warp bytes, warps
 #ifdef FUEL_PROF
   double end_prof_us[3];  // the last fuelgpu_frontier_search_end: stream wait, result assembly, closing event (host µs)
@@ -231,6 +232,15 @@ int poly_waypoints_impl(FuelMap* m, int B, int w_max, const int32_t* n_wp_dev, c
 // astar.cu: Astar::search + shortenPath + planExploreMotion's goal branch (fast_exploration_manager.cpp:238-263)
 int astar_impl(FuelMap* m, int B, const double* start_dev, const double* goal_dev, const FuelAstarParams* p,
                FuelPathInfo* info_dev, int path_max, double* path_dev, int w_max, int32_t* nwp_dev, double* wp_dev);
+// the same search as ViewNode::searchPath runs it, over the queries list_dev[0 .. *n_list_dev) of P pairs: getPath() and
+// its pathLength, no shortenPath or branch; the node pool is clamped to what max_iter can use
+int astar_raw_impl(FuelMap* m, int P, const int* n_list_dev, const int* list_dev, const double* p1_dev,
+                   const double* p2_dev, const FuelAstarParams* p, FuelPathInfo* info_dev, int path_max,
+                   double* path_dev);
+// view_cost.cu: ViewNode::searchPath + computeCost (graph_node.cpp:32-85) for P pairs
+int view_cost_impl(FuelMap* m, int P, const double* p1, const double* p2, const double* y1, const double* y2,
+                   const double* v1, const FuelViewCostParams* vp, FuelViewCostInfo* info_dev, int path_max,
+                   double* path_dev);
 
 // getDistWithGrad on the device (sdf_map.cpp:497-536); shared by esdf.cu and bspline.cu
 __device__ __forceinline__ double dev_get_distance(const Geom& g, const float* __restrict__ dist,

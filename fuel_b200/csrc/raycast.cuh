@@ -22,6 +22,9 @@ __device__ __forceinline__ double intbound(double s, double ds) {  // raycast.cp
 
 // RayCaster::input(start, end) then nextId until the end voxel (raycast.cpp:329-394); blocked by an inflated-occupied or
 // UNKNOWN voxel (voxels outside the map read -1 in the reference: neither).  Returns true when the ray is clear.
+// kBox: a voxel outside the exploration box blocks too (!isInBox(idx), sdf_map.h:171-178), as ViewNode::searchPath's
+// straight-line test has it (graph_node.cpp:36-43).
+template <bool kBox = false>
 __device__ bool ray_is_clear(const Geom& g, const uint8_t* __restrict__ occ, const double start[3], const double end[3]) {
   const double res = g.res;
   const double s0 = start[0] / res, s1 = start[1] / res, s2 = start[2] / res;
@@ -56,6 +59,9 @@ __device__ bool ray_is_clear(const Geom& g, const uint8_t* __restrict__ occ, con
       const uint8_t o = occ[addr_of(g, ix, iy, iz)];
       if ((o & 4) || (o & 3) == FUELGPU_UNKNOWN) return false;
     }
+    if (kBox && (ix < g.box_min[0] || ix >= g.box_max[0] || iy < g.box_min[1] || iy >= g.box_max[1] ||
+                 iz < g.box_min[2] || iz >= g.box_max[2]))
+      return false;
   }
   return true;
 }

@@ -6,13 +6,17 @@ active_perception/src/frontier_finder.cpp:23-121 (file:line under /root/referenc
 isFrontierChanged :365-372, removed_ids_) on the host and every voxel-scale step in
 libfuelgpu.  The step right after it (SURVEY.md 8f rank 4) is mirrored too: computeFrontiersToVisit
 (:392-423) with sampleViewpoints / countVisibleCells (:662-695,734-755) on the device, and
-isFrontierCovered (:697-719).  The cost matrix / TSP (updateFrontierCostMatrix etc.) stay out of scope.
+isFrontierCovered (:697-719).  So is the tour's cost bookkeeping: updateFrontierCostMatrix (:260-326),
+getFullCostMatrix (:531-592, the asymmetric form the reference runs) and getPathForTour (:508-529), each edge a
+ViewNode::computeCost / searchPath of fuel_b200.view_node, all the edges of one call in one device batch.  The TSP
+solver itself (LKH) is not part of this library.
 """
 import ctypes as C
 
 import numpy as np
 
 from ._lib import FuelFrontierParams, FuelViewParams, check, lib, ptr
+from .view_node import ViewNode
 
 
 def _data(a):
@@ -22,7 +26,8 @@ def _data(a):
 
 class Frontier:
     """frontier_finder.h:34-51"""
-    __slots__ = ("cells_addr_", "filtered_cells_", "average_", "id_", "box_min_", "box_max_", "_map", "viewpoints_")
+    __slots__ = ("cells_addr_", "filtered_cells_", "average_", "id_", "box_min_", "box_max_", "_map", "viewpoints_",
+                 "costs_", "paths_")
 
     def __init__(self, m, addr, filtered, average, box_min, box_max):
         self._map = m
@@ -33,6 +38,8 @@ class Frontier:
         self.box_max_ = box_max
         self.id_ = -1
         self.viewpoints_ = []  # [(pos_ [3], yaw_, visib_num_)], frontier_finder.h:25-31
+        self.costs_ = []  # computeCost to every cluster, in frontiers_ order (frontier_finder.h:49-50)
+        self.paths_ = []  # searchPath's path to every cluster, [n, 3] arrays
 
     @property
     def cells_(self):
@@ -42,6 +49,63 @@ class Frontier:
         nyz = m.shape[1] * m.shape[2]
         idx = np.stack([a // nyz, (a % nyz) // m.shape[2], a % m.shape[2]], axis=1)
         return (idx + 0.5) * m.resolution_ + m.map_origin_
+
+
+def update_cost_matrix(frontiers, first_new, removed_ids, cost_batch):
+    """updateFrontierCostMatrix (frontier_finder.cpp:260-326) over a frontier list whose clusters from index first_new
+    on are new (None: none).  cost_batch(p1, p2, y1, y2, v1) -> (cost [P], paths) costs every old x new and new x new
+    pair in one call; the lists grow in the reference's order."""
+    first = len(frontiers) if first_new is None else first_new
+    if removed_ids:  # the ids are indices after the removal (:75-84), so erase one after another (:267-286)
+        for f in frontiers[:first]:
+            for r in removed_ids:
+                del f.costs_[r]
+                del f.paths_[r]
+    pairs = [(i, j) for i in range(first) for j in range(first, len(frontiers))]
+    pairs += [(i, j) for i in range(first, len(frontiers)) for j in range(i, len(frontiers))]
+    edges = [(i, j) for i, j in pairs if i != j]
+    cost, paths = [], []
+    if edges:
+        vi = [frontiers[i].viewpoints_[0] for i, _ in edges]
+        vj = [frontiers[j].viewpoints_[0] for _, j in edges]
+        cost, paths = cost_batch([v[0] for v in vi], [v[0] for v in vj], [v[1] for v in vi], [v[1] for v in vj],
+                                 np.zeros((len(edges), 3)))
+    k = 0
+    for i, j in pairs:
+        if i == j:
+            frontiers[i].costs_.append(0.0)
+            frontiers[i].paths_.append(np.zeros((0, 3)))
+            continue
+        frontiers[i].costs_.append(float(cost[k]))
+        frontiers[i].paths_.append(paths[k])
+        frontiers[j].costs_.append(float(cost[k]))
+        frontiers[j].paths_.append(paths[k][::-1].copy())
+        k += 1
+
+
+def full_cost_matrix(frontiers, cur_pos, cur_vel, cur_yaw, cost_batch):
+    """getFullCostMatrix's asymmetric form (frontier_finder.cpp:562-591): [n + 1, n + 1], the clusters' cost lists in
+    rows 1..n, column 0 zero, row 0 the cost from the current state (cur_yaw = (yaw, yaw rate, -)) in one call"""
+    n = len(frontiers)
+    mat = np.zeros((n + 1, n + 1))
+    for i, f in enumerate(frontiers):
+        mat[i + 1, 1:1 + len(f.costs_)] = f.costs_
+    mat[:, 0] = 0.0
+    if n:
+        views = [f.viewpoints_[0] for f in frontiers]
+        cost, _ = cost_batch(np.repeat(np.asarray(cur_pos, np.float64).reshape(1, 3), n, axis=0),
+                             [v[0] for v in views], np.full(n, float(cur_yaw[0])), [v[1] for v in views],
+                             np.repeat(np.asarray(cur_vel, np.float64).reshape(1, 3), n, axis=0))
+        mat[0, 1:] = cost
+    return mat
+
+
+def path_for_tour(frontiers, pos, frontier_ids, cost_batch):
+    """getPathForTour (frontier_finder.cpp:508-529): searchPath from pos to the first cluster's top viewpoint, then the
+    stored paths along the tour -> [n, 3]"""
+    _, paths = cost_batch([pos], [frontiers[frontier_ids[0]].viewpoints_[0][0]], [0.0], [0.0], np.zeros((1, 3)))
+    segs = [paths[0]] + [frontiers[a].paths_[b] for a, b in zip(frontier_ids[:-1], frontier_ids[1:])]
+    return np.concatenate([np.asarray(s, np.float64).reshape(-1, 3) for s in segs])
 
 
 class FrontierFinder:
@@ -292,6 +356,27 @@ class FrontierFinder:
             if c >= max(thresh, 1):  # `++change_num >= change_thresh` fires on a changed cell only
                 return True
         return False
+
+    # ---- the tour's cost: each edge as ViewNode's statics say, searched on this finder's map ----
+    def _cost_batch(self):
+        def batch(p1, p2, y1, y2, v1):
+            cost, _, paths = ViewNode.costBatch(p1, p2, y1, y2, v1, sdf_map=self._map)
+            return cost, paths
+        return batch
+
+    def updateFrontierCostMatrix(self):
+        """frontier_finder.cpp:260-326: drop the removed clusters from the old cost lists, then cost every old x new
+        and new x new pair of viewpoints in one device batch"""
+        update_cost_matrix(self.frontiers_, self.first_new_ftr_, self.removed_ids_, self._cost_batch())
+        self.removed_ids_ = []
+
+    def getFullCostMatrix(self, cur_pos, cur_vel, cur_yaw):
+        """frontier_finder.cpp:531-592 (the asymmetric TSP form) -> [n + 1, n + 1]"""
+        return full_cost_matrix(self.frontiers_, cur_pos, cur_vel, cur_yaw, self._cost_batch())
+
+    def getPathForTour(self, pos, frontier_ids):
+        """frontier_finder.cpp:508-529 -> [n, 3]"""
+        return path_for_tour(self.frontiers_, pos, frontier_ids, self._cost_batch())
 
     def getFrontiers(self):
         return [f.cells_ for f in self.frontiers_]

@@ -425,3 +425,26 @@ def make_path_queries(g, inflate, tri, B=1024, seed=20261017):
         start[b], goal[b], kind[b] = s, q, k
         b += 1
     return dict(start=start, goal=goal, kind=kind)
+
+
+def make_view_pairs(g, inflate, tri, P=4096, seed=20261018):
+    """Viewpoint pairs for ViewNode::computeCost (graph_node.cpp:63-85) as the tour's cost asks for them: the pairs of
+    make_path_queries (clear and blocked lines, goals in unknown or occupied space, start == goal), one in eight with
+    its second point moved above the exploration box so that the line leaves it, yaws over the whole circle, and a
+    velocity on half of the pairs -- some below the 1e-3 threshold and some along the pair's own direction, where
+    acos meets a dot product at 1.  Returns dict(p1, p2, v1 [P, 3], y1, y2 [P])."""
+    rng = np.random.default_rng(seed)
+    q = make_path_queries(g, inflate, tri, B=P, seed=seed)
+    p1, p2 = q["start"].copy(), q["goal"].copy()
+    out = rng.uniform(size=P) < 0.125
+    p2[out, 2] = g.box_max[2] + rng.uniform(0.05, 0.5, int(out.sum()))
+    y1, y2 = rng.uniform(-np.pi, np.pi, P), rng.uniform(-np.pi, np.pi, P)
+    v1 = np.zeros((P, 3))
+    r = rng.uniform(size=P)
+    moving = r < 0.4
+    v1[moving] = rng.normal(size=(int(moving.sum()), 3)) * np.array([1.0, 1.0, 0.3])
+    tiny = (r >= 0.4) & (r < 0.45)
+    v1[tiny] = rng.normal(size=(int(tiny.sum()), 3)) * 3e-4
+    along = (r >= 0.45) & (r < 0.5)
+    v1[along] = (p2[along] - p1[along]) * rng.uniform(0.2, 2.0, (int(along.sum()), 1))
+    return dict(p1=p1, p2=p2, y1=y1, y2=y2, v1=v1)

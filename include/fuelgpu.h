@@ -647,6 +647,52 @@ FUELGPU_API int fuelgpu_astar_batch_dev(FuelMap* map, int32_t B, const void* sta
                                         const FuelAstarParams* params, void* info_dev, int32_t path_max, void* path_dev,
                                         int32_t w_max, void* n_wp_dev, void* waypts_dev);
 
+/* ---- tour cost between viewpoints: ViewNode::searchPath and ViewNode::computeCost on the device -------------------
+ * For P pairs (p1, p2, y1, y2, v1), what ViewNode::computeCost(p1, p2, y1, y2, v1, 0, path)
+ * (active_perception/src/graph_node.cpp:63-85) returns and the path ViewNode::searchPath (:32-61) leaves: the edge cost
+ * of FrontierFinder::updateFrontierCostMatrix (frontier_finder.cpp:260-326, v1 = 0) and of getFullCostMatrix's first
+ * row (:562-591, v1 = the current velocity).  Per pair:
+ *   1. the straight line p1 -> p2: the RayCaster walk of the viewpoint visibility (input, then nextId until the end
+ *      voxel), blocked by an inflated-occupied, UNKNOWN or outside-the-box voxel (!isInBox(idx)).  Clear: kind LINE,
+ *      path {p1, p2}, length (p1 - p2).norm().  Like every ray walk of this library it gives up after 4096 voxels and
+ *      counts the line clear (the reference's loop has no bound);
+ *   2. a blocked line: Astar::search(p1, p2) at params->astar (as fuelgpu_astar_batch searches, iteration cap and all;
+ *      the reference sets resolution 0.4).  REACH_END: kind ASTAR, path getPath() (start ... end node, goal; no
+ *      shortenPath), length Astar::pathLength of it.  Otherwise kind NO_PATH, path {p1, p2}, length 1000;
+ *   3. cost = max(length / vm [+ w_dir * acos(v1.normalized() . (p2 - p1).normalized()) when |v1| > 1e-3],
+ *      min(|y2 - y1|, 2 pi - |y2 - y1|) / yd), std::max's NaN behaviour included.
+ * Every output but cost equals the reference's fp64 arithmetic bit for bit; cost too wherever |v1| <= 1e-3.  acos is
+ * the device's (within 2 ulp of the correctly rounded value), so with a velocity the cost may differ in its last bits.
+ *   p1, p2, v1 [P][3], y1, y2 [P]; params: vm, yd finite and > 0, w_dir finite, astar as fuelgpu_astar_batch checks it
+ * Outputs: info [P]; path [P][path_max][3] or NULL: its first path_max rows, zero past them.  A row with a non-finite
+ * input gets kind 0, reason FUELGPU_ASTAR_BAD_INPUT and zeros; the other rows are unaffected (both entries).
+ * Scratch: the search's (fuelgpu_astar_batch) with the node pool clamped to min(allocate_num, 26 * max_iter + 2) -- a
+ * search never uses more, so the results are those of allocate_num -- plus about 256 + 76 * P bytes.  Runs on the map's main
+ * stream with no host synchronisation inside (the search reads the blocked pairs' count from device memory); the host
+ * entry waits once, at the end. */
+#define FUELGPU_VIEW_LINE 1    /* the straight line is clear */
+#define FUELGPU_VIEW_ASTAR 2   /* the line is blocked, A* reached the goal */
+#define FUELGPU_VIEW_NO_PATH 3 /* the line is blocked, A* did not reach it: length 1000 */
+typedef struct {
+  double vm, yd, w_dir;  /* ViewNode::vm_, yd_, w_dir_ (exploration/vm, exploration/yd, exploration/w_dir) */
+  FuelAstarParams astar; /* ViewNode::astar_: the astar/ parameters, resolution as searchPath sets it (0.4) */
+} FuelViewCostParams;
+typedef struct {
+  int32_t kind;                     /* FUELGPU_VIEW_LINE / ASTAR / NO_PATH, 0 on a bad row */
+  int32_t reason;                   /* the search's FuelPathInfo.reason (ASTAR, NO_PATH), FUELGPU_ASTAR_BAD_INPUT */
+  int32_t iter_num, use_node_num;   /* the search's (ASTAR, NO_PATH), else 0 */
+  int32_t n_path, reserved;         /* path.size() */
+  double length;                    /* searchPath's return value */
+  double cost;                      /* computeCost's return value */
+} FuelViewCostInfo;
+FUELGPU_API int fuelgpu_view_cost_batch(FuelMap* map, int32_t P, const double* p1, const double* p2, const double* y1,
+                                        const double* y2, const double* v1, const FuelViewCostParams* params,
+                                        FuelViewCostInfo* info, int32_t path_max, double* path);
+FUELGPU_API int fuelgpu_view_cost_batch_dev(FuelMap* map, int32_t P, const void* p1_dev, const void* p2_dev,
+                                            const void* y1_dev, const void* y2_dev, const void* v1_dev,
+                                            const FuelViewCostParams* params, void* info_dev, int32_t path_max,
+                                            void* path_dev);
+
 /* ---- multi-GPU: the z-sharded ESDF update (BASELINE config 4; SURVEY 8e row 1) ---------------------------
  * Multi-GPU form of SDFMap::updateESDF3d (plan_env/src/sdf_map.cpp:152-241) over the whole map.  One process
  * (or thread) per GPU; rank r owns planes [r*nz/G, (r+1)*nz/G) of every (x,y) column, z fastest like the
