@@ -98,6 +98,10 @@ class FuelViewCostParams(C.Structure):
     _fields_ = [("vm", C.c_double), ("yd", C.c_double), ("w_dir", C.c_double), ("astar", FuelAstarParams)]
 
 
+class FuelLocalTourParams(C.Structure):
+    _fields_ = [("view", FuelViewCostParams), ("tour_lambda_heu", C.c_double)]
+
+
 class FuelTrajReport(C.Structure):
     _fields_ = [("duration", C.c_double), ("jerk", C.c_double), ("ratio", C.c_double), ("distance", C.c_double),
                 ("safe", C.c_int32), ("feasible", C.c_int32), ("n_checked", C.c_int32), ("reserved", C.c_int32)]
@@ -200,6 +204,10 @@ SIGNATURES = {
                                           _vp]),
     "fuelgpu_view_cost_batch_dev": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp, _vp, C.POINTER(FuelViewCostParams), _vp,
                                               _i32, _vp]),
+    "fuelgpu_local_tour_batch": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.POINTER(FuelLocalTourParams),
+                                           _vp, _i32, _vp, _i32, _vp, _vp]),
+    "fuelgpu_local_tour_batch_dev": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                               C.POINTER(FuelLocalTourParams), _vp, _i32, _vp, _i32, _vp, _vp]),
 }
 
 _lib = None

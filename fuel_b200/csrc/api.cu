@@ -275,6 +275,7 @@ int fuelgpu_map_destroy(FuelMap* m) {
   m->tc_buf.release();
   m->as_buf.release();
   m->vc_buf.release();
+  m->lt_buf.release();
   for (int t = 0; t < T_COUNT; ++t) {
     if (m->ev0[t]) cudaEventDestroy(m->ev0[t]);
     if (m->ev1[t]) cudaEventDestroy(m->ev1[t]);
@@ -1348,4 +1349,100 @@ int fuelgpu_view_cost_batch(FuelMap* m, int32_t P, const double* p1, const doubl
   return st.download();
 }
 
+// The structure of a local-tour batch: returns 0 and the group, viewpoint and edge counts, or FUELGPU_EINVAL.
+static int check_local_tour_args(FuelMap* m, int32_t B, const int32_t* prob_off, const int32_t* group_off,
+                                 const FuelLocalTourParams* p, int32_t kmax, int32_t tour_max, const void* cur_pos,
+                                 const void* cur_vel, const void* cur_yaw, const void* vp_pos, const void* vp_yaw,
+                                 const void* info, const void* refined, const void* tour, int32_t* G_out,
+                                 int32_t* N_out, int64_t* E_out) {
+  if (!m) return fuel_fail(nullptr, FUELGPU_EINVAL, "null map");
+  if (B < 0) return fuel_fail(m, FUELGPU_EINVAL, "negative batch");
+  if (!p) return fuel_fail(m, FUELGPU_EINVAL, "null params");
+  const int rc = check_view_cost_args(m, 0, nullptr, nullptr, nullptr, nullptr, nullptr, &p->view, nullptr, 0, nullptr);
+  if (rc) return rc;
+  if (!isfinite(p->tour_lambda_heu)) return fuel_fail(m, FUELGPU_EINVAL, "tour_lambda_heu must be finite");
+  if (tour_max < 1) return fuel_fail(m, FUELGPU_EINVAL, "tour_max must be at least 1");
+  if (kmax < 1) return fuel_fail(m, FUELGPU_EINVAL, "kmax must be at least 1");
+  *G_out = 0, *N_out = 0, *E_out = 0;
+  if (B == 0) return 0;
+  if (!prob_off || !group_off || !cur_pos || !cur_vel || !cur_yaw || !info || !refined || !tour)
+    return fuel_fail(m, FUELGPU_EINVAL, "null argument");
+  if (prob_off[0] != 0) return fuel_fail(m, FUELGPU_EINVAL, "prob_off[0] must be 0");
+  for (int32_t b = 0; b < B; ++b) {
+    const int32_t ng = prob_off[b + 1] - prob_off[b];
+    if (prob_off[b + 1] < prob_off[b] || ng < 1)
+      return fuel_fail(m, FUELGPU_EINVAL, "problem %s%lld has no group", "", (long long)b);
+    if (ng > kmax) return fuel_fail(m, FUELGPU_EINVAL, "problem %s%lld has more groups than kmax", "", (long long)b);
+  }
+  const int32_t G = prob_off[B];
+  if (group_off[0] != 0) return fuel_fail(m, FUELGPU_EINVAL, "group_off[0] must be 0");
+  for (int32_t g = 0; g < G; ++g)
+    if (group_off[g + 1] < group_off[g]) return fuel_fail(m, FUELGPU_EINVAL, "group_off decreases at %s%lld", "", g);
+  int64_t E = 0;
+  for (int32_t b = 0; b < B; ++b) {
+    const int32_t g0 = prob_off[b], ng = prob_off[b + 1] - g0;
+    if (group_off[g0 + ng] == group_off[g0 + ng - 1])  // final_node would stay null (fast_exploration_manager.cpp:460)
+      return fuel_fail(m, FUELGPU_EINVAL, "problem %s%lld: the last group is empty", "", (long long)b);
+    int64_t nodes = 1, n_in = 1;
+    for (int32_t i = 0; i < ng; ++i) {
+      const int64_t sz = group_off[g0 + i + 1] - group_off[g0 + i], eff = i == ng - 1 ? 1 : sz;
+      nodes += eff;
+      E += eff * n_in;
+      n_in = eff;
+    }
+    if (nodes > FUELGPU_TOUR_MAX_NODES)
+      return fuel_fail(m, FUELGPU_EINVAL, "problem %s%lld has more than FUELGPU_TOUR_MAX_NODES nodes", "", (long long)b);
+  }
+  if (E > INT32_MAX / 2) return fuel_fail(m, FUELGPU_EINVAL, "too many edges in one batch");
+  if (G > 0 && (int64_t)G * tour_max > INT32_MAX / 4) return fuel_fail(m, FUELGPU_EINVAL, "groups * tour_max too large");
+  if (group_off[G] > 0 && (!vp_pos || !vp_yaw)) return fuel_fail(m, FUELGPU_EINVAL, "null argument");
+  *G_out = G, *N_out = group_off[G], *E_out = E;
+  return 0;
+}
+
+int fuelgpu_local_tour_batch_dev(FuelMap* m, int32_t B, const int32_t* prob_off, const int32_t* group_off,
+                                 const void* cur_pos_dev, const void* cur_vel_dev, const void* cur_yaw_dev,
+                                 const void* vp_pos_dev, const void* vp_yaw_dev, const FuelLocalTourParams* p,
+                                 void* info_dev, int32_t kmax, void* refined_dev, int32_t tour_max, void* tour_dev,
+                                 void* edge_cost_dev) {
+  int32_t G, N;
+  int64_t E;
+  int rc = check_local_tour_args(m, B, prob_off, group_off, p, kmax, tour_max, cur_pos_dev, cur_vel_dev, cur_yaw_dev,
+                                 vp_pos_dev, vp_yaw_dev, info_dev, refined_dev, tour_dev, &G, &N, &E);
+  if (rc || B == 0) return rc;
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  const LocalTourIO io{ (const double*)cur_pos_dev, (const double*)cur_vel_dev, (const double*)cur_yaw_dev,
+                        (const double*)vp_pos_dev, (const double*)vp_yaw_dev, (FuelLocalTourInfo*)info_dev,
+                        (int32_t*)refined_dev, (double*)tour_dev, (double*)edge_cost_dev, kmax, tour_max };
+  return local_tour_impl(m, B, prob_off, group_off, p, io);
+}
+
+int fuelgpu_local_tour_batch(FuelMap* m, int32_t B, const int32_t* prob_off, const int32_t* group_off,
+                             const double* cur_pos, const double* cur_vel, const double* cur_yaw, const double* vp_pos,
+                             const double* vp_yaw, const FuelLocalTourParams* p, FuelLocalTourInfo* info, int32_t kmax,
+                             int32_t* refined, int32_t tour_max, double* tour, double* edge_cost) {
+  int32_t G, N;
+  int64_t E;
+  int rc = check_local_tour_args(m, B, prob_off, group_off, p, kmax, tour_max, cur_pos, cur_vel, cur_yaw, vp_pos,
+                                 vp_yaw, info, refined, tour, &G, &N, &E);
+  if (rc || B == 0) return rc;
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  const size_t nb = (size_t)B, nn = (size_t)N;
+  double *d_pos, *d_vel, *d_yaw, *d_vpp, *d_vpy, *d_tour, *d_ec;
+  FuelLocalTourInfo* d_info;
+  int32_t* d_ref;
+  HostStaging st(m);
+  st.in(&d_pos, cur_pos, nb * 3).in(&d_vel, cur_vel, nb * 3).in(&d_yaw, cur_yaw, nb);
+  st.in(&d_vpp, vp_pos, nn * 3).in(&d_vpy, vp_yaw, nn);
+  st.out(&d_info, info, nb).out(&d_ref, refined, nb * kmax).out(&d_tour, tour, nb * tour_max * 3);
+  st.out(&d_ec, edge_cost, (size_t)E);
+  rc = st.upload();
+  if (rc) return rc;
+  const LocalTourIO io{ d_pos, d_vel, d_yaw, d_vpp, d_vpy, d_info, d_ref, d_tour, d_ec, kmax, tour_max };
+  rc = local_tour_impl(m, B, prob_off, group_off, p, io);
+  if (rc) return rc;
+  return st.download();
+}
+
 }  // extern "C"
+

@@ -8,6 +8,7 @@
 // parallel; lane 0 then applies the state updates (node allocation, g / f, parent, heap push) serially in loop order.
 // Built with -fmad=false: every double operation rounds as the reference's does.
 #include "common.cuh"
+#include "heap.cuh"
 #include "raycast.cuh"
 
 #include <math.h>
@@ -89,38 +90,6 @@ __device__ int table_insert(Slot* tab, unsigned mask, const int id[3], int w) {
   while (tab[s].w >= 0) s = (s + 1) & mask;
   tab[s] = Slot{ id[0], id[1], id[2], w };
   return (int)s;
-}
-
-// std::priority_queue<NodePtr, vector, NodeComparator0>::push / pop as libstdc++ implements them (push_heap,
-// pop_heap -> __adjust_heap -> __push_heap), comparing node1->f_score > node2->f_score through the current f of each id
-__device__ void heap_sift_up(int* heap, const double* f, int hole, int v) {
-  const double fv = f[v];
-  int parent = (hole - 1) / 2;
-  while (hole > 0 && f[heap[parent]] > fv) {
-    heap[hole] = heap[parent];
-    hole = parent;
-    parent = (hole - 1) / 2;
-  }
-  heap[hole] = v;
-}
-__device__ void heap_pop(int* heap, int len, const double* f) {
-  if (len <= 1) return;
-  const int n = len - 1;
-  const int v = heap[n];
-  heap[n] = heap[0];
-  int hole = 0, child = 0;
-  while (child < (n - 1) / 2) {
-    child = 2 * (child + 1);
-    if (f[heap[child]] > f[heap[child - 1]]) child--;
-    heap[hole] = heap[child];
-    hole = child;
-  }
-  if ((n & 1) == 0 && child == (n - 2) / 2) {
-    child = 2 * (child + 1);
-    heap[hole] = heap[child - 1];
-    hole = child - 1;
-  }
-  heap_sift_up(heap, f, hole, v);
 }
 
 struct NbrShared {  // one warp's 26 neighbour results, written in parallel and consumed by lane 0 in loop order

@@ -88,6 +88,7 @@ struct FuelMap {
   DevBuf<uint8_t> tc_buf;  // the other host-facing batch calls (check, evaluate, parameterize, poly, yaw, A*, esdf_sample)
   DevBuf<uint8_t> as_buf;  // A* search scratch (astar.cu)
   DevBuf<uint8_t> vc_buf;  // view cost: the blocked-line list and the searches' results (view_cost.cu)
+  DevBuf<uint8_t> lt_buf;  // local tour: the graph, its edges and their costs, the search state, the tour segments
   size_t as_stride, as_warps;  // layout whose key tables are known empty: per-warp bytes, warps
 #ifdef FUEL_PROF
   double end_prof_us[3];  // the last fuelgpu_frontier_search_end: stream wait, result assembly, closing event (host µs)
@@ -241,6 +242,16 @@ int astar_raw_impl(FuelMap* m, int P, const int* n_list_dev, const int* list_dev
 int view_cost_impl(FuelMap* m, int P, const double* p1, const double* p2, const double* y1, const double* y2,
                    const double* v1, const FuelViewCostParams* vp, FuelViewCostInfo* info_dev, int path_max,
                    double* path_dev);
+// local_tour.cu: refineLocalTour (fast_exploration_manager.cpp:429-503) for B problems; prob_off / group_off on the host
+struct LocalTourIO {
+  const double *cur_pos, *cur_vel, *cur_yaw, *vp_pos, *vp_yaw;  // device
+  FuelLocalTourInfo* info;
+  int32_t* refined;
+  double *tour, *edge_cost;  // edge_cost may be null
+  int kmax, tour_max;
+};
+int local_tour_impl(FuelMap* m, int B, const int32_t* prob_off, const int32_t* group_off, const FuelLocalTourParams* p,
+                    const LocalTourIO& io);
 
 // getDistWithGrad on the device (sdf_map.cpp:497-536); shared by esdf.cu and bspline.cu
 __device__ __forceinline__ double dev_get_distance(const Geom& g, const float* __restrict__ dist,

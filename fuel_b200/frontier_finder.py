@@ -336,6 +336,32 @@ class FrontierFinder:
             avgs.append(f.average_)
         return pts, yaws, avgs
 
+    def getViewpointsInfo(self, cur_pos, ids, view_num, max_decay, min_candidate_dist=0.75):
+        """frontier_finder.cpp:452-484: for each id (a cluster of that id_; none, no entry) its first viewpoints,
+        at most view_num, while visib_num_ stays above int(front visib_num_ * max_decay), skipping those closer than
+        min_candidate_dist; when that leaves none, the same without the distance limit -> (points, yaws) lists"""
+        points, yaws = [], []
+        cur_pos = np.asarray(cur_pos, dtype=np.float64)
+        for fid in ids:
+            for f in self.frontiers_:
+                if f.id_ != fid:
+                    continue
+                thresh = int(f.viewpoints_[0][2] * max_decay)  # int visib_thresh = visib_num_ * max_decay
+                pts, ys = [], []
+                for far_only in (True, False):
+                    for v in f.viewpoints_:
+                        if len(pts) >= view_num or v[2] <= thresh:
+                            break
+                        if far_only and np.linalg.norm(v[0] - cur_pos) < min_candidate_dist:
+                            continue
+                        pts.append(v[0].copy())
+                        ys.append(v[1])
+                    if pts:
+                        break
+                points.append(pts)
+                yaws.append(ys)
+        return points, yaws
+
     def isFrontierCovered(self):
         """frontier_finder.cpp:697-719: has any stored cluster overlapping the updated box lost at least
         min_view_finish_fraction_ of its cells?"""

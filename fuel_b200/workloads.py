@@ -448,3 +448,68 @@ def make_view_pairs(g, inflate, tri, P=4096, seed=20261018):
     along = (r >= 0.45) & (r < 0.5)
     v1[along] = (p2[along] - p1[along]) * rng.uniform(0.2, 2.0, (int(along.sum()), 1))
     return dict(p1=p1, p2=p2, y1=y1, y2=y2, v1=v1)
+
+
+def make_local_tours(g, inflate, tri, B=256, seed=20261019):
+    """refineLocalTour problems (fast_exploration_manager.cpp:429-503) as planExploreMotion builds them: a current
+    state in known-free space and 2 to 7 groups of 1 to 15 viewpoints, each group spread 1.5 to 2.5 m around a point
+    2 to 6 m on from the one before (some in unknown or occupied space, so lines are blocked and searches fail).
+    Half the problems move; among them some fly exactly along the first edge (acos at a dot product of 1).  The
+    special cases, one problem in twelve each: duplicated viewpoints (equal g values), a group of one repeated
+    viewpoint (all its costs equal), an empty middle group (unreachable), a first group of one viewpoint at cur_pos
+    (a zero-length tour segment), a single group.
+    Returns dict(prob_off [B+1], group_off [G+1], cur_pos, cur_vel [B, 3], cur_yaw [B], vp_pos [N, 3], vp_yaw [N],
+    kind [B]: 0 plain, 1 duplicates, 2 repeated group, 3 empty middle group, 4 refined point at cur_pos, 5 one group)."""
+    rng = np.random.default_rng(seed)
+    pool = make_path_queries(g, inflate, tri, B=4 * B + 64, seed=seed)["start"]
+    prob_off, group_off = [0], [0]
+    cur_pos, cur_vel, cur_yaw, vp_pos, vp_yaw, kinds = [], [], [], [], [], []
+    for b in range(B):
+        kind = int(rng.integers(12)) if rng.uniform() < 0.5 else 0
+        kind = kind if kind <= 5 else 0
+        p0 = pool[rng.integers(len(pool))]
+        ng = 1 if kind == 5 else int(rng.integers(2, 8))
+        c = p0.copy()
+        groups = []
+        for i in range(ng):
+            d = np.linalg.norm(pool - c, axis=1)
+            near = np.flatnonzero((d > 2.0) & (d < 6.0))
+            c = pool[rng.choice(near)] if len(near) else c
+            n = int(rng.integers(1, 16))
+            phi = rng.uniform(-np.pi, np.pi, n)
+            r = rng.uniform(1.5, 2.5, n)
+            pts = c + np.stack([r * np.cos(phi), r * np.sin(phi), rng.uniform(-0.3, 0.3, n)], axis=1)
+            ys = rng.uniform(-np.pi, np.pi, n)
+            groups.append([pts, ys])
+        if kind == 1:  # duplicates: repeat viewpoints inside groups
+            for grp in groups[:-1]:
+                k = rng.integers(len(grp[0]), size=max(1, len(grp[0]) // 2))
+                grp[0], grp[1] = np.concatenate([grp[0], grp[0][k]]), np.concatenate([grp[1], grp[1][k]])
+        elif kind == 2 and ng > 1:  # one group of a single repeated viewpoint
+            i = int(rng.integers(ng - 1))
+            n = len(groups[i][0])
+            groups[i] = [np.repeat(groups[i][0][:1], n, axis=0), np.repeat(groups[i][1][:1], n)]
+        elif kind == 3 and ng > 2:
+            groups[int(rng.integers(1, ng - 1))] = [np.zeros((0, 3)), np.zeros(0)]
+        elif kind == 4 and ng > 1:
+            groups[0] = [p0.reshape(1, 3).copy(), groups[0][1][:1]]
+        for pts, ys in groups:
+            vp_pos.append(pts)
+            vp_yaw.append(ys)
+            group_off.append(group_off[-1] + len(pts))
+        prob_off.append(prob_off[-1] + ng)
+        v = np.zeros(3)
+        u = rng.uniform()
+        if u < 0.35:
+            v = rng.normal(size=3) * np.array([1.0, 1.0, 0.3])
+        elif u < 0.45 and len(groups[0][0]):  # along the edge to the first group's first viewpoint
+            v = (groups[0][0][0] - p0) * rng.uniform(0.2, 2.0)
+        elif u < 0.5:
+            v = rng.normal(size=3) * 3e-4
+        cur_pos.append(p0)
+        cur_vel.append(v)
+        cur_yaw.append(rng.uniform(-np.pi, np.pi))
+        kinds.append(kind)
+    return dict(prob_off=np.asarray(prob_off, np.int32), group_off=np.asarray(group_off, np.int32),
+                cur_pos=np.asarray(cur_pos), cur_vel=np.asarray(cur_vel), cur_yaw=np.asarray(cur_yaw),
+                vp_pos=np.concatenate(vp_pos), vp_yaw=np.concatenate(vp_yaw), kind=np.asarray(kinds, np.int32))

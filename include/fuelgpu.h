@@ -693,6 +693,76 @@ FUELGPU_API int fuelgpu_view_cost_batch_dev(FuelMap* map, int32_t P, const void*
                                             const FuelViewCostParams* params, void* info_dev, int32_t path_max,
                                             void* path_dev);
 
+/* ---- local tour refinement: FastExplorationManager::refineLocalTour on the device ---------------------------------
+ * B independent refineLocalTour(cur_pos, cur_vel, cur_yaw, n_points, n_yaws, refined_pts, refined_yaws) problems
+ * (exploration_manager/src/fast_exploration_manager.cpp:429-503).  Problem b has groups prob_off[b] .. prob_off[b+1]
+ * (n_points / n_yaws, in order); group g has viewpoints vp_pos / vp_yaw [group_off[g] .. group_off[g+1]).  As the
+ * reference builds it: node 0 is the current state (vel_ = cur_vel, yaw cur_yaw[b]), every viewpoint of a group is a
+ * node with zero velocity, except that the last group keeps only its first viewpoint (final_node); each node of a group
+ * has an edge from every node of the group before (node 0 for the first group), in addEdge order: group, new node,
+ * then previous-group node.  Each edge costs ViewNode::computeCost (fuelgpu_view_cost_batch, eagerly, all at once);
+ * DijkstraSearch (graph_search.h:76-118) then runs over that table exactly as the reference's std::priority_queue does
+ * it (g_value_ from 1e6, strict <, neighbours in order, stale entries popped and expanded again).  refined holds the
+ * viewpoints of path[1..] as indices into vp_*; the tour is ed_->refined_tour_: cur_pos, then for each refined point
+ * ViewNode::searchPath from the tour's end with astar.lambda_heu = tour_lambda_heu, its path appended when searchPath
+ * returns nonzero (NaN and 1000 included), the point alone otherwise.
+ * The reference evaluates costTo lazily, as Dijkstra expands nodes; costTo is a pure function of its pair, so every
+ * output is the reference's given the same edge costs.  n_evals is the number of costTo calls the reference makes.
+ * Divergences are those of fuelgpu_view_cost_batch: the iteration cap for max_search_time, the 4096-voxel ray guard,
+ * and the device's acos on node 0's edges when |cur_vel| > 1e-3 (g may then differ in its last bits).
+ *   prob_off [B + 1], group_off [G + 1]: HOST memory in both entries, starting at 0 and nondecreasing.
+ *   cur_pos, cur_vel [B][3], cur_yaw [B], vp_pos [N][3], vp_yaw [N]: host arrays, device pointers in _dev.
+ *   params: view as fuelgpu_view_cost_batch checks it (resolution 0.4 as searchPath sets it), tour_lambda_heu finite
+ *   (refineLocalTour sets 1.0 for the tour's searches).
+ * Outputs (host arrays, device pointers in _dev): info [B]; refined [B][kmax], -1 past n_refined; tour
+ * [B][tour_max][3], zero past n_tour; edge_cost [E] or NULL: every edge's cost in addEdge order, problem by problem.
+ * Status per problem:
+ *   FUELGPU_TOUR_OK;
+ *   FUELGPU_TOUR_UNREACHABLE: the open set ran empty before final_node was popped (an empty middle group, or edges of
+ *     NaN or >= 1e6 cost): n_refined 0, g 1e6, tour [cur_pos] -- the reference then indexes refined_points_[0], which
+ *     is undefined behaviour;
+ *   FUELGPU_TOUR_BAD_INPUT: a non-finite cur_pos / cur_vel / cur_yaw or graph node coordinate: everything zero, refined
+ *     -1; the other problems are unaffected.  Its tour segments go to the searches as non-finite rows, which cost none;
+ *   FUELGPU_TOUR_TRUNCATED: as OK, but the tour needs n_tour > tour_max rows; the first tour_max are written.  Call
+ *     again with tour_max >= n_tour.
+ * FUELGPU_EINVAL, nothing written: B < 0, a problem with no group or an empty last group (the reference dereferences a
+ * null final_node), more than FUELGPU_TOUR_MAX_NODES nodes or more than kmax groups in one problem, tour_max < 1, a
+ * bad parameter or a null argument.
+ * Runs on the map's main stream with no host synchronisation inside: the edge enumeration, the edge costs
+ * (fuelgpu_view_cost_batch's three launches), the search (one warp per problem), the tour's segment costs (again the
+ * view-cost launches), the tour assembly.  The host entry waits once, at the end.
+ * Scratch: one map-owned device buffer grown on demand, about 164 E + 16 N' + 28 B + 188 G + 24 G tour_max bytes
+ * (E edges, N' graph nodes, G groups), plus the view-cost scratch of fuelgpu_view_cost_batch. */
+#define FUELGPU_TOUR_MAX_NODES 1024
+#define FUELGPU_TOUR_OK 0
+#define FUELGPU_TOUR_UNREACHABLE 1
+#define FUELGPU_TOUR_BAD_INPUT 2
+#define FUELGPU_TOUR_TRUNCATED 3
+typedef struct {
+  FuelViewCostParams view; /* ViewNode's statics: the edge costs and the tour's searches */
+  double tour_lambda_heu;  /* ViewNode::astar_->lambda_heu_ for the tour's searches (refineLocalTour :490: 1.0) */
+} FuelLocalTourParams;
+typedef struct {
+  int32_t status;          /* FUELGPU_TOUR_OK ... FUELGPU_TOUR_TRUNCATED */
+  int32_t n_nodes, n_edges; /* the graph's node_num_ and edge_num_ */
+  int32_t n_evals;         /* costTo calls the reference's lazy search makes */
+  int32_t n_refined;       /* refined_pts.size() */
+  int32_t n_tour;          /* ed_->refined_tour_.size() (the rows needed when TRUNCATED) */
+  int32_t pops, pushes;    /* open-set pops and pushes (the start's push included) */
+  double g;                /* final_node's g_value_ */
+} FuelLocalTourInfo;
+FUELGPU_API int fuelgpu_local_tour_batch(FuelMap* map, int32_t B, const int32_t* prob_off, const int32_t* group_off,
+                                         const double* cur_pos, const double* cur_vel, const double* cur_yaw,
+                                         const double* vp_pos, const double* vp_yaw, const FuelLocalTourParams* params,
+                                         FuelLocalTourInfo* info, int32_t kmax, int32_t* refined, int32_t tour_max,
+                                         double* tour, double* edge_cost);
+FUELGPU_API int fuelgpu_local_tour_batch_dev(FuelMap* map, int32_t B, const int32_t* prob_off,
+                                             const int32_t* group_off, const void* cur_pos_dev,
+                                             const void* cur_vel_dev, const void* cur_yaw_dev, const void* vp_pos_dev,
+                                             const void* vp_yaw_dev, const FuelLocalTourParams* params,
+                                             void* info_dev, int32_t kmax, void* refined_dev, int32_t tour_max,
+                                             void* tour_dev, void* edge_cost_dev);
+
 /* ---- multi-GPU: the z-sharded ESDF update (BASELINE config 4; SURVEY 8e row 1) ---------------------------
  * Multi-GPU form of SDFMap::updateESDF3d (plan_env/src/sdf_map.cpp:152-241) over the whole map.  One process
  * (or thread) per GPU; rank r owns planes [r*nz/G, (r+1)*nz/G) of every (x,y) column, z fastest like the

@@ -469,6 +469,7 @@ struct FrontierParam {  // frontier_finder.cpp:29-40
   int cluster_min_ = 100;
   double cluster_size_xy_ = 2.0;
   int down_sample_ = 3;
+  double min_candidate_dist_ = 0.75;  // frontier/min_candidate_dist (getTopViewpointsInfo, getViewpointsInfo)
 };
 
 class FrontierFinder {
@@ -642,6 +643,43 @@ public:
     }
   }
 
+  // getTopViewpointsInfo (frontier_finder.cpp:425-450): each cluster's first viewpoint at least min_candidate_dist_
+  // away, else its first
+  void getTopViewpointsInfo(const Vector3d& cur_pos, std::vector<Vector3d>& points, std::vector<double>& yaws,
+                            std::vector<Vector3d>& averages) const {
+    points.clear(), yaws.clear(), averages.clear();
+    for (const auto& f : frontiers_) {
+      const Viewpoint* v = &f.viewpoints_.front();  // all too close: the first (highest coverage)
+      for (const auto& w : f.viewpoints_) {
+        if (dist(w.pos_, cur_pos) < p_.min_candidate_dist_) continue;
+        v = &w;
+        break;
+      }
+      points.push_back(v->pos_), yaws.push_back(v->yaw_), averages.push_back(f.average_);
+    }
+  }
+  // getViewpointsInfo (frontier_finder.cpp:452-484): for each id, up to view_num viewpoints while visib_num_ stays above
+  // int(front visib_num_ * max_decay), the too-close ones skipped unless that leaves none
+  void getViewpointsInfo(const Vector3d& cur_pos, const std::vector<int>& ids, const int& view_num,
+                         const double& max_decay, std::vector<std::vector<Vector3d>>& points,
+                         std::vector<std::vector<double>>& yaws) const {
+    points.clear(), yaws.clear();
+    for (int id : ids)
+      for (const auto& f : frontiers_) {
+        if (f.id_ != id) continue;
+        std::vector<Vector3d> pts;
+        std::vector<double> ys;
+        const int visib_thresh = f.viewpoints_.front().visib_num_ * max_decay;
+        for (int pass = 0; pass < 2 && pts.empty(); ++pass)
+          for (const auto& v : f.viewpoints_) {
+            if ((int)pts.size() >= view_num || v.visib_num_ <= visib_thresh) break;
+            if (pass == 0 && dist(v.pos_, cur_pos) < p_.min_candidate_dist_) continue;
+            pts.push_back(v.pos_), ys.push_back(v.yaw_);
+          }
+        points.push_back(pts), yaws.push_back(ys);
+      }
+  }
+
   void getFrontiers(std::vector<std::vector<Vector3d>>& clusters) const {
     clusters.clear();
     for (auto& f : frontiers_) clusters.push_back(f.cells_);
@@ -656,6 +694,10 @@ public:
 
 private:
   FuelMap* gpu() const { return edt_env_->sdf_map_->gpu(); }
+  static double dist(const Vector3d& a, const Vector3d& b) {  // (a - b).norm()
+    const double x = a(0) - b(0), y = a(1) - b(1), z = a(2) - b(2);
+    return std::sqrt((x * x + y * y) + z * z);
+  }
   static bool haveOverlap(const Vector3d& min1, const Vector3d& max1, const Vector3d& min2, const Vector3d& max2) {
     for (int i = 0; i < 3; ++i) {  // frontier_finder.cpp:353-363
       const double bmin = std::max(min1[i], min2[i]), bmax = std::min(max1[i], max2[i]);
@@ -695,6 +737,69 @@ private:
   std::shared_ptr<EDTEnvironment> edt_env_;
   FrontierParam p_;
 };
+
+// ---- FastExplorationManager's local tour (fast_exploration_manager.cpp:129-216, 429-503) --------------------------
+// refineLocalTour with the reference's arguments plus ed_->refined_tour_, in one fuelgpu_local_tour_batch call with
+// ViewNode's statics.  Returns the FUELGPU_TOUR_* status: FUELGPU_TOUR_UNREACHABLE leaves refined_pts empty and the tour
+// {cur_pos}, where the reference's caller reads refined_points_[0] of an empty vector.  n_points must have at least one
+// group and a nonempty last group (the reference dereferences a null final_node otherwise).  Afterwards
+// ViewNode::astar_param_.lambda_heu is 10000, as the reference leaves ViewNode::astar_->lambda_heu_ (:499).
+inline int refineLocalTour(const Vector3d& cur_pos, const Vector3d& cur_vel, const Vector3d& cur_yaw,
+                           const std::vector<std::vector<Vector3d>>& n_points,
+                           const std::vector<std::vector<double>>& n_yaws, std::vector<Vector3d>& refined_pts,
+                           std::vector<double>& refined_yaws, std::vector<Vector3d>& refined_tour) {
+  FuelMap* h = ViewNode::map_->gpu();
+  const int32_t G = (int32_t)n_points.size();
+  std::vector<int32_t> group_off(1, 0);
+  std::vector<double> vp, vy;
+  for (int i = 0; i < G; ++i) {
+    for (size_t j = 0; j < n_points[i].size(); ++j)
+      vp.insert(vp.end(), { n_points[i][j](0), n_points[i][j](1), n_points[i][j](2) }), vy.push_back(n_yaws[i][j]);
+    group_off.push_back((int32_t)vy.size());
+  }
+  const int32_t prob_off[2] = { 0, G };
+  const auto& a = ViewNode::astar_param_;
+  const FuelLocalTourParams prm{ { ViewNode::vm_, ViewNode::yd_, ViewNode::w_dir_,
+                                   { 0.4, a.lambda_heu, a.allocate_num, a.max_iter } },
+                                 1.0 };  // ViewNode::astar_->lambda_heu_ = 1.0 for the tour (:490)
+  FuelLocalTourInfo info;
+  std::vector<int32_t> refined(std::max(G, 1));
+  std::vector<double> tour;
+  for (int32_t tour_max = 256;;) {  // a tour longer than tour_max rows: run again with room for it
+    tour.assign(3 * (size_t)tour_max, 0.0);
+    fuelgpu_check(fuelgpu_local_tour_batch(h, 1, prob_off, group_off.data(), cur_pos.data(), cur_vel.data(),
+                                           &cur_yaw(0), vp.data(), vy.data(), &prm, &info, std::max(G, 1),
+                                           refined.data(), tour_max, tour.data(), nullptr),
+                  h);
+    if (info.status != FUELGPU_TOUR_TRUNCATED) break;
+    tour_max = info.n_tour;
+  }
+  refined_pts.clear(), refined_yaws.clear(), refined_tour.clear();
+  for (int i = 0; i < info.n_refined; ++i)
+    refined_pts.push_back(Vector3d(vp[3 * refined[i]], vp[3 * refined[i] + 1], vp[3 * refined[i] + 2])),
+        refined_yaws.push_back(vy[refined[i]]);
+  for (int i = 0; i < info.n_tour; ++i) refined_tour.push_back(Vector3d(tour[3 * i], tour[3 * i + 1], tour[3 * i + 2]));
+  ViewNode::astar_param_.lambda_heu = 10000;  // ViewNode::astar_->lambda_heu_ = 10000 (:499)
+  return info.status;
+}
+
+// planExploreMotion's one-frontier pick (:202-214): the first strict minimum of computeCost(pos, p, yaw[0], y, vel)
+// below 100000 over the frontier's viewpoints, in one ViewNode::costBatch call; -1 when there is none (the reference
+// then indexes n_points_[0][-1])
+inline int pickOneViewpoint(const Vector3d& pos, const Vector3d& vel, const Vector3d& yaw,
+                            const std::vector<Vector3d>& points, const std::vector<double>& yaws) {
+  if (points.empty()) return -1;
+  const size_t n = points.size();
+  std::vector<double> cost;
+  std::vector<std::vector<Vector3d>> paths;
+  ViewNode::costBatch(std::vector<Vector3d>(n, pos), points, std::vector<double>(n, yaw(0)), yaws,
+                      std::vector<Vector3d>(n, vel), cost, paths);
+  double min_cost = 100000;
+  int min_cost_id = -1;
+  for (size_t i = 0; i < n; ++i)
+    if (cost[i] < min_cost) min_cost = cost[i], min_cost_id = (int)i;
+  return min_cost_id;
+}
 
 // ---- BsplineOptimizer (bspline_optimizer.h:20-145) -------------------------------------------------
 class BsplineOptimizer {
