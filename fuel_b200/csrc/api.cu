@@ -211,6 +211,7 @@ int fuelgpu_map_create(const FuelGridDesc* grid, int device_id, FuelMap** out) {
   m->stream = m->own_stream;
   CR(cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking));
   CR(cudaEventCreateWithFlags(&m->copy_ev, cudaEventDisableTiming));
+  CR(cudaEventCreateWithFlags(&m->mirror_ev, cudaEventDisableTiming));
   CR(cudaStreamCreateWithFlags(&m->in_stream, cudaStreamNonBlocking));
   CR(cudaEventCreateWithFlags(&m->in_ev, cudaEventDisableTiming));
   for (int t = 0; t < T_COUNT; ++t) {
@@ -285,6 +286,7 @@ int fuelgpu_map_destroy(FuelMap* m) {
     cudaStreamDestroy(m->copy_stream);
   }
   if (m->copy_ev) cudaEventDestroy(m->copy_ev);
+  if (m->mirror_ev) cudaEventDestroy(m->mirror_ev);
   if (m->in_stream) {
     cudaStreamSynchronize(m->in_stream);
     cudaStreamDestroy(m->in_stream);
@@ -512,6 +514,7 @@ int fuelgpu_esdf_update(FuelMap* m, const int32_t bmin[3], const int32_t bmax[3]
   int rc = check_box(m, bmin, bmax, lo, hi);
   if (rc) return rc;
   FUEL_CUDA(m, cudaSetDevice(m->dev));
+  esdf_order_writer(m);
   tbegin(m, T_ESDF);
   rc = esdf_update_impl(m, lo, hi, flags);
   tend(m, T_ESDF);
@@ -552,6 +555,7 @@ int fuelgpu_esdf_set_from_slabs_dev(FuelMap* m, const void* slabs_dev, int32_t n
   if (!m || !slabs_dev) return fuel_fail(m, FUELGPU_EINVAL, "null argument");
   if (n_slabs < 1 || m->g.nz % n_slabs) return fuel_fail(m, FUELGPU_EINVAL, "nz is not a multiple of the slab count");
   FUEL_CUDA(m, cudaSetDevice(m->dev));
+  esdf_order_writer(m);
   if (n_slabs == 1) {
     FUEL_CUDA(m, cudaMemcpyAsync(m->dist, slabs_dev, sizeof(float) * m->nvox, cudaMemcpyDeviceToDevice, m->stream));
   } else {
@@ -582,6 +586,8 @@ int fuelgpu_esdf_download_async(FuelMap* m, const int32_t bmin[3], const int32_t
   tbegin(m, T_DOWNLOAD, m->copy_stream);
   FUEL_CUDA(m, cudaMemcpyAsync(out_f32 + off, m->dist + off, cnt * 4, cudaMemcpyDeviceToHost, m->copy_stream));
   tend(m, T_DOWNLOAD, m->copy_stream);
+  FUEL_CUDA(m, cudaEventRecord(m->mirror_ev, m->copy_stream));
+  m->mirror_pending = true;
   return 0;
 }
 

@@ -71,6 +71,8 @@ struct FuelMap {
   cudaStream_t copy_stream;  // D2H mirror copies that may overlap the main stream
   cudaEvent_t copy_ev;
   bool dist_ev_ok;           // ev1[T_ESDF] marks the last write of `dist` (a mirror download waits on it, not on later work)
+  cudaEvent_t mirror_ev;     // end of the last mirror download on copy_stream: writers of `dist` on the main stream wait for it
+  bool mirror_pending;
   cudaStream_t in_stream;    // H2D of the solver inputs: goes out at once, not behind the ESDF kernels of the main stream
   cudaEvent_t in_ev;
   cudaEvent_t ev0[T_COUNT], ev1[T_COUNT];
@@ -175,6 +177,10 @@ void fusion_get_updated_box(FuelMap* m, double bmin[3], double bmax[3], int rese
 void fusion_state_destroy(FuelMap* m);
 double* fusion_logodds_ptr(FuelMap* m, double* clamp_max_log);
 void frontier_order_writer(FuelMap* m);
+// main-stream writers of `dist` wait for an enqueued mirror download (fuelgpu_esdf_download_async)
+static inline void esdf_order_writer(FuelMap* m) {
+  if (m->mirror_pending) cudaStreamWaitEvent(m->stream, m->mirror_ev, 0);
+}
 int frontier_set_cell_order(FuelMap* m, int order);
 int frontier_candidates_impl(FuelMap* m, const double umin[3], const double umax[3], const FuelFrontierParams* p, int z_lo,
                              int z_hi, int32_t* n_out);

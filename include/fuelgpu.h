@@ -182,7 +182,9 @@ FUELGPU_API int fuelgpu_esdf_download(FuelMap* map, const int32_t bmin[3], const
                           float* out_f32, double* out_f64);
 /* Same for float32, without blocking: the copy is queued on the handle's copy stream behind the
  * ESDF update and overlaps whatever runs next on the main stream (the trajectory batch); the host
- * buffer is valid after fuelgpu_map_synchronize().  Use with a page-locked buffer. */
+ * buffer is valid after fuelgpu_map_synchronize().  Later writers of the field on the main stream
+ * (fuelgpu_esdf_update, fuelgpu_esdf_set_from_slabs_dev) wait for the copy, so the buffer holds the
+ * field as it was when this call was made.  Use with a page-locked buffer. */
 FUELGPU_API int fuelgpu_esdf_download_async(FuelMap* map, const int32_t bmin[3], const int32_t bmax[3],
                                 float* out_f32);
 /* Replaces SDFMap::getDistWithGrad (sdf_map.cpp:497-536) = EDTEnvironment::evaluateEDTWithGrad
