@@ -208,6 +208,8 @@ SIGNATURES = {
                                            _vp, _i32, _vp, _i32, _vp, _vp]),
     "fuelgpu_local_tour_batch_dev": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                                C.POINTER(FuelLocalTourParams), _vp, _i32, _vp, _i32, _vp, _vp]),
+    "fuelgpu_global_tour_batch": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp]),
+    "fuelgpu_global_tour_batch_dev": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

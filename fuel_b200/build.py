@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libfuelgpu.so")
 SOURCES = ["api.cu", "esdf.cu", "esdf_tile.cu", "sharded.cu", "frontier.cu", "bspline.cu", "bspline_solve.cu", "bspline_solve_long.cu",
            "fusion.cu", "viewpoints.cu", "traj_check.cu", "poly_traj.cu", "astar.cu",
-           "view_cost.cu", "local_tour.cu"]
+           "view_cost.cu", "local_tour.cu", "global_tour.cu"]
 FMAD_OK = {"bspline_solve.cu", "bspline_solve_long.cu", "esdf.cu", "esdf_tile.cu", "sharded.cu"}  # files whose arithmetic need not follow the host rounding sequence
 HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "bspline_eval.cuh"), os.path.join(CSRC, "raycast.cuh"),
            os.path.join(CSRC, "heap.cuh"), os.path.join(ROOT, "include", "fuelgpu.h")]

@@ -277,6 +277,7 @@ int fuelgpu_map_destroy(FuelMap* m) {
   m->as_buf.release();
   m->vc_buf.release();
   m->lt_buf.release();
+  m->gt_buf.release();
   for (int t = 0; t < T_COUNT; ++t) {
     if (m->ev0[t]) cudaEventDestroy(m->ev0[t]);
     if (m->ev1[t]) cudaEventDestroy(m->ev1[t]);
@@ -1446,6 +1447,51 @@ int fuelgpu_local_tour_batch(FuelMap* m, int32_t B, const int32_t* prob_off, con
   if (rc) return rc;
   const LocalTourIO io{ d_pos, d_vel, d_yaw, d_vpp, d_vpy, d_info, d_ref, d_tour, d_ec, kmax, tour_max };
   rc = local_tour_impl(m, B, prob_off, group_off, p, io);
+  if (rc) return rc;
+  return st.download();
+}
+
+// The shape of a global-tour batch: returns 0 and the matrix and index entry counts, or FUELGPU_EINVAL.
+static int check_global_tour_args(FuelMap* m, int32_t B, const int32_t* dims, const void* cost, const void* info,
+                                  const void* indices, int64_t* n_cost, int64_t* n_idx) {
+  if (!m) return fuel_fail(nullptr, FUELGPU_EINVAL, "null map");
+  if (B < 0) return fuel_fail(m, FUELGPU_EINVAL, "negative batch");
+  *n_cost = 0, *n_idx = 0;
+  if (B == 0) return 0;
+  if (!dims || !cost || !info || !indices) return fuel_fail(m, FUELGPU_EINVAL, "null argument");
+  for (int32_t b = 0; b < B; ++b) {
+    const int64_t d = dims[b];
+    if (d < 2) return fuel_fail(m, FUELGPU_EINVAL, "instance %s%lld has no cluster (dims < 2)", "", (long long)b);
+    if (*n_cost > (INT64_MAX >> 4) - d * d) return fuel_fail(m, FUELGPU_EINVAL, "matrices too large");
+    *n_cost += d * d;
+    *n_idx += d - 1;
+  }
+  return 0;
+}
+
+int fuelgpu_global_tour_batch_dev(FuelMap* m, int32_t B, const int32_t* dims, const void* cost_dev, void* info_dev,
+                                  void* indices_dev) {
+  int64_t nc, ni;
+  const int rc = check_global_tour_args(m, B, dims, cost_dev, info_dev, indices_dev, &nc, &ni);
+  if (rc || B == 0) return rc;
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  return global_tour_impl(m, B, dims, (const double*)cost_dev, (FuelGlobalTourInfo*)info_dev, (int32_t*)indices_dev);
+}
+
+int fuelgpu_global_tour_batch(FuelMap* m, int32_t B, const int32_t* dims, const double* cost,
+                              FuelGlobalTourInfo* info, int32_t* indices) {
+  int64_t nc, ni;
+  int rc = check_global_tour_args(m, B, dims, cost, info, indices, &nc, &ni);
+  if (rc || B == 0) return rc;
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  double* d_cost;
+  FuelGlobalTourInfo* d_info;
+  int32_t* d_idx;
+  HostStaging st(m);
+  st.in(&d_cost, cost, (size_t)nc).out(&d_info, info, (size_t)B).out(&d_idx, indices, (size_t)ni);
+  rc = st.upload();
+  if (rc) return rc;
+  rc = global_tour_impl(m, B, dims, d_cost, d_info, d_idx);
   if (rc) return rc;
   return st.download();
 }

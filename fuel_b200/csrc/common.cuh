@@ -91,6 +91,7 @@ struct FuelMap {
   DevBuf<uint8_t> as_buf;  // A* search scratch (astar.cu)
   DevBuf<uint8_t> vc_buf;  // view cost: the blocked-line list and the searches' results (view_cost.cu)
   DevBuf<uint8_t> lt_buf;  // local tour: the graph, its edges and their costs, the search state, the tour segments
+  DevBuf<uint8_t> gt_buf;  // global tour: the instance table and the Held-Karp tables of one group (global_tour.cu)
   size_t as_stride, as_warps;  // layout whose key tables are known empty: per-warp bytes, warps
 #ifdef FUEL_PROF
   double end_prof_us[3];  // the last fuelgpu_frontier_search_end: stream wait, result assembly, closing event (host µs)
@@ -258,6 +259,9 @@ struct LocalTourIO {
 };
 int local_tour_impl(FuelMap* m, int B, const int32_t* prob_off, const int32_t* group_off, const FuelLocalTourParams* p,
                     const LocalTourIO& io);
+// global_tour.cu: findGlobalTour's ATSP (fast_exploration_manager.cpp:327-427) for B instances; dims on the host
+int global_tour_impl(FuelMap* m, int B, const int32_t* dims, const double* cost_dev, FuelGlobalTourInfo* info_dev,
+                     int32_t* indices_dev);
 
 // getDistWithGrad on the device (sdf_map.cpp:497-536); shared by esdf.cu and bspline.cu
 __device__ __forceinline__ double dev_get_distance(const Geom& g, const float* __restrict__ dist,

@@ -1,5 +1,8 @@
-"""The local tour of FastExplorationManager::planExploreMotion (exploration_manager/src/fast_exploration_manager.cpp:
-88-293) on the device, between the global tour and the path to the next viewpoint.
+"""The global and local tours of FastExplorationManager::planExploreMotion (exploration_manager/src/
+fast_exploration_manager.cpp:88-293) on the device, between the frontier cost matrix and the path to the next viewpoint.
+
+findGlobalTour (:327-427) solves the ATSP over getFullCostMatrix's matrix that the reference hands to LKH; here
+global_tour_batch solves it exactly on the device (fuelgpu_global_tour_batch, up to GTOUR_MAX_CLUSTERS clusters).
 
 With refine_local the reference takes the first frontiers of the global tour (select_refined_ids, :139-147), fetches up
 to top_view_num viewpoints of each (FrontierFinder.getViewpointsInfo) and picks one per frontier with refineLocalTour
@@ -23,6 +26,13 @@ TOUR_MAX_NODES = 1024
 TOUR_INFO_DTYPE = np.dtype([("status", np.int32), ("n_nodes", np.int32), ("n_edges", np.int32),
                             ("n_evals", np.int32), ("n_refined", np.int32), ("n_tour", np.int32), ("pops", np.int32),
                             ("pushes", np.int32), ("g", np.float64)])
+
+# FuelGlobalTourInfo.status
+GTOUR_OK, GTOUR_BAD_INPUT, GTOUR_TOO_LARGE = 0, 1, 2
+GTOUR_MAX_CLUSTERS = 20
+# one FuelGlobalTourInfo per instance (include/fuelgpu.h)
+GTOUR_INFO_DTYPE = np.dtype([("status", np.int32), ("n", np.int32), ("n_optimal", np.int32), ("reserved", np.int32),
+                             ("cost", np.int64)])
 
 
 @dataclass
@@ -138,3 +148,38 @@ def pick_one_viewpoint(pos, points, yaws, vel, yaw, sdf_map=None):
         if c < min_cost:
             min_cost, min_id = c, i
     return min_id
+
+
+def global_tour_batch(sdf_map, dims, cost):
+    """fuelgpu_global_tour_batch over B instances -> (info [B] of GTOUR_INFO_DTYPE, indices [sum(dims - 1)]): the raw
+    arrays the C entry writes.  Instance b is the dims[b] x dims[b] matrix at its place in `cost` (the matrices
+    concatenated, row-major); its tour is the dims[b] - 1 cluster ids at its place in `indices` (-1 unless OK)."""
+    dims = np.ascontiguousarray(dims, np.int32).reshape(-1)
+    cost = np.ascontiguousarray(np.asarray(cost, np.float64).reshape(-1))
+    B = len(dims)
+    info = np.zeros(B, dtype=GTOUR_INFO_DTYPE)
+    indices = np.zeros(max(int(dims.astype(np.int64).sum()) - B, 0), np.int32)
+    h = _handle(sdf_map)
+    check(lib().fuelgpu_global_tour_batch(h, B, ptr(dims), ptr(cost), ptr(info), ptr(indices)), h)
+    return info, indices
+
+
+def findGlobalTour(frontier_finder, cur_pos, cur_vel, cur_yaw):
+    """fast_exploration_manager.cpp:327-427 -> (indices, global_tour [k, 3]): updateFrontierCostMatrix, then
+    getFullCostMatrix, then the tour LKH would be asked for, solved exactly in one device call (the lexicographically
+    smallest of the optimal tours), then getPathForTour.  Raises ValueError where the matrix has a cost whose int(cost *
+    100) is undefined (NaN, infinite, out of int32) and where there are more than GTOUR_MAX_CLUSTERS clusters (such a
+    caller keeps LKH)."""
+    ff = frontier_finder
+    ff.updateFrontierCostMatrix()
+    mat = ff.getFullCostMatrix(cur_pos, cur_vel, cur_yaw)
+    if mat.shape[0] < 2:
+        raise ValueError("findGlobalTour: no frontier")
+    info, indices = global_tour_batch(ff._map, [mat.shape[0]], mat)
+    if info["status"][0] == GTOUR_BAD_INPUT:
+        raise ValueError("findGlobalTour: a cost whose integer conversion is undefined (NaN, inf or beyond int32)")
+    if info["status"][0] == GTOUR_TOO_LARGE:
+        raise ValueError("findGlobalTour: %d clusters, more than GTOUR_MAX_CLUSTERS = %d" % (mat.shape[0] - 1,
+                                                                                          GTOUR_MAX_CLUSTERS))
+    ids = [int(i) for i in indices]
+    return ids, ff.getPathForTour(cur_pos, ids)

@@ -513,3 +513,32 @@ def make_local_tours(g, inflate, tri, B=256, seed=20261019):
     return dict(prob_off=np.asarray(prob_off, np.int32), group_off=np.asarray(group_off, np.int32),
                 cur_pos=np.asarray(cur_pos), cur_vel=np.asarray(cur_vel), cur_yaw=np.asarray(cur_yaw),
                 vp_pos=np.concatenate(vp_pos), vp_yaw=np.concatenate(vp_yaw), kind=np.asarray(kinds, np.int32))
+
+
+def make_global_tours(n, B=1, seed=20261020, kind="geometric", vm=2.0, yd=60 * 3.1415926 / 180.0):
+    """B cost matrices of findGlobalTour's shape ([B, n + 1, n + 1], column 0 zero) for the global tour:
+    "geometric": ViewNode::computeCost's form over random viewpoints of a 20 x 20 x 3 m box, max(distance / vm,
+    yaw change / yd), one pair in ten at the 1000 of a failed search (in both directions, as updateFrontierCostMatrix
+    stores it), row 0 from a current state with a velocity term; "random": integer-valued costs 0 .. 19.99 with one
+    entry in five at 500 (an asymmetric matrix with far outliers)."""
+    rng = np.random.default_rng(seed)
+    d = n + 1
+    out = np.zeros((B, d, d))
+    for b in range(B):
+        if kind == "random":
+            m = rng.integers(0, 2000, (d, d)) / 100.0
+            m[rng.random((d, d)) < 0.2] = 500.0
+        else:
+            p = rng.uniform([0, 0, 0], [20, 20, 3], (d, 3))
+            y = rng.uniform(-3.1415926, 3.1415926, d)
+            dist = np.linalg.norm(p[:, None] - p[None], axis=2)
+            dy = np.abs(y[:, None] - y[None])
+            dy = np.minimum(dy, 2 * 3.1415926 - dy)
+            m = np.maximum(dist / vm, dy / yd)
+            fail = np.triu(rng.random((d, d)) < 0.1, 1)
+            m[fail | fail.T] = 1000.0
+            m[0, 1:] += rng.uniform(0, 0.5, n)  # the velocity change from the current state
+        m[:, 0] = 0.0
+        np.fill_diagonal(m, 0.0)
+        out[b] = m
+    return out

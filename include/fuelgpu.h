@@ -765,6 +765,49 @@ FUELGPU_API int fuelgpu_local_tour_batch_dev(FuelMap* map, int32_t B, const int3
                                              void* info_dev, int32_t kmax, void* refined_dev, int32_t tour_max,
                                              void* tour_dev, void* edge_cost_dev);
 
+/* ---- global tour: the ATSP of FastExplorationManager::findGlobalTour, solved exactly on the device -----------------
+ * findGlobalTour (exploration_manager/src/fast_exploration_manager.cpp:327-427) writes getFullCostMatrix's
+ * (n + 1) x (n + 1) matrix as a TSPLIB ATSP, solves it with LKH and reads the tour back.  These entries solve the same
+ * problem for B instances exactly (Held-Karp dynamic programming over subsets), so no tour is worse than LKH's.
+ * Instance b has dimension d_b = dims[b] = n + 1: node 0 is the current state, nodes 1 .. n the clusters; its matrix
+ * is d_b x d_b row-major doubles in `cost`, the instances concatenated.
+ *   - Integer costs as the reference makes them: int(cost(i, j) * 100), the double product truncated toward zero
+ *     (:357-376).  The diagonal is never read.
+ *   - Objective: LKH's cycle cost c[0][t1] + c[t1][t2] + ... + c[tn][0], summed in int64.  getFullCostMatrix's column 0
+ *     is zero, so in FUEL this is the open tour from the current state.
+ *   - Output: indices (the instance's n entries in the concatenation) are the 0-based cluster ids t1 - 1 .. tn - 1, as
+ *     findGlobalTour pushes id - 2 for LKH's 1-based node id.  Among optimal tours, the lexicographically smallest
+ *     sequence.  info.cost is the optimal cost, info.n_optimal the number of optimal tours (saturating at INT32_MAX).
+ *   - n = 1 gives [0] (the reference calls findGlobalTour only for more than one cluster; LKH rejects dimension < 3).
+ * Status per instance; the others are unaffected:
+ *   FUELGPU_GTOUR_OK;
+ *   FUELGPU_GTOUR_BAD_INPUT: an off-diagonal product that is NaN, infinite or whose truncation does not fit int32
+ *     (undefined behaviour in the reference's conversion);
+ *   FUELGPU_GTOUR_TOO_LARGE: n > FUELGPU_GTOUR_MAX_CLUSTERS; such a caller keeps LKH.
+ *   For both, info holds only status and n, and the indices are -1.
+ * FUELGPU_EINVAL, nothing written: B < 0, a dims[b] < 2 (n < 1), or a null argument while B > 0.
+ *   dims [B]: HOST memory in both entries, so the host sizes everything without a read-back.
+ *   cost [sum d_b^2], info [B], indices [sum (d_b - 1)]: host arrays, device pointers in _dev.
+ * Runs on the map's main stream with no host synchronisation inside; the host entry waits once, at the end.  Scratch:
+ * one map-owned device buffer grown on demand: a 32 B descriptor and a 4 B status per instance (each array rounded up
+ * to 256 B), plus, per group of instances, the sum of 4 (n+1)^2 + 12 n 2^n bytes per instance (each part rounded up to
+ * 256 B; about 252 MB at n = 20, 2.8 MB at n = 14), groups of at most 4 GiB. */
+#define FUELGPU_GTOUR_MAX_CLUSTERS 20
+#define FUELGPU_GTOUR_OK 0
+#define FUELGPU_GTOUR_BAD_INPUT 1
+#define FUELGPU_GTOUR_TOO_LARGE 2
+typedef struct {
+  int32_t status;    /* FUELGPU_GTOUR_OK ... FUELGPU_GTOUR_TOO_LARGE */
+  int32_t n;         /* clusters: dims[b] - 1 */
+  int32_t n_optimal; /* optimal tours, saturating at INT32_MAX */
+  int32_t reserved;  /* 0 */
+  int64_t cost;      /* the optimal tour's cost in the integer units above */
+} FuelGlobalTourInfo;
+FUELGPU_API int fuelgpu_global_tour_batch(FuelMap* map, int32_t B, const int32_t* dims, const double* cost,
+                                          FuelGlobalTourInfo* info, int32_t* indices);
+FUELGPU_API int fuelgpu_global_tour_batch_dev(FuelMap* map, int32_t B, const int32_t* dims, const void* cost_dev,
+                                              void* info_dev, void* indices_dev);
+
 /* ---- multi-GPU: the z-sharded ESDF update (BASELINE config 4; SURVEY 8e row 1) ---------------------------
  * Multi-GPU form of SDFMap::updateESDF3d (plan_env/src/sdf_map.cpp:152-241) over the whole map.  One process
  * (or thread) per GPU; rank r owns planes [r*nz/G, (r+1)*nz/G) of every (x,y) column, z fastest like the

@@ -801,6 +801,28 @@ inline int pickOneViewpoint(const Vector3d& pos, const Vector3d& vel, const Vect
   return min_cost_id;
 }
 
+// FastExplorationManager::findGlobalTour (:327-427) over the finder's frontier list: updateFrontierCostMatrix,
+// getFullCostMatrix, then the ATSP it writes for LKH solved exactly in one fuelgpu_global_tour_batch call (the
+// lexicographically smallest optimal tour), then getPathForTour into global_tour.  Returns the FUELGPU_GTOUR_* status;
+// on FUELGPU_GTOUR_BAD_INPUT (a cost whose int(cost * 100) is undefined) and FUELGPU_GTOUR_TOO_LARGE (more than
+// FUELGPU_GTOUR_MAX_CLUSTERS clusters: keep LKH for such a list) indices and global_tour are left empty.
+inline int findGlobalTour(FrontierFinder& ff, const Vector3d& cur_pos, const Vector3d& cur_vel,
+                          const Vector3d& cur_yaw, std::vector<int>& indices, std::vector<Vector3d>& global_tour) {
+  FuelMap* h = ViewNode::map_->gpu();  // the map the finder's costs are searched on
+  ff.updateFrontierCostMatrix();
+  std::vector<double> mat;
+  ff.getFullCostMatrix(cur_pos, cur_vel, cur_yaw, mat);
+  const int32_t dim = (int32_t)ff.frontiers_.size() + 1;
+  FuelGlobalTourInfo info;
+  std::vector<int32_t> ids((size_t)dim - 1);
+  fuelgpu_check(fuelgpu_global_tour_batch(h, 1, &dim, mat.data(), &info, ids.data()), h);
+  indices.clear(), global_tour.clear();
+  if (info.status != FUELGPU_GTOUR_OK) return info.status;
+  indices.assign(ids.begin(), ids.end());
+  ff.getPathForTour(cur_pos, indices, global_tour);
+  return info.status;
+}
+
 // ---- BsplineOptimizer (bspline_optimizer.h:20-145) -------------------------------------------------
 class BsplineOptimizer {
 public:
