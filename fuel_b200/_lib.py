@@ -94,6 +94,12 @@ class FuelAstarParams(C.Structure):
                 ("max_iter", C.c_int32)]
 
 
+class FuelKinoParams(C.Structure):
+    _fields_ = [(k, C.c_double) for k in ("max_tau", "init_max_tau", "max_vel", "vel_margin", "max_acc", "w_time",
+                                          "horizon", "lambda_heu", "resolution", "ctrl_pt_dist", "manager_max_vel")] + \
+               [(k, C.c_int32) for k in ("allocate_num", "check_num", "optimistic", "reserved")]
+
+
 class FuelViewCostParams(C.Structure):
     _fields_ = [("vm", C.c_double), ("yd", C.c_double), ("w_dir", C.c_double), ("astar", FuelAstarParams)]
 
@@ -210,6 +216,10 @@ SIGNATURES = {
                                                C.POINTER(FuelLocalTourParams), _vp, _i32, _vp, _i32, _vp, _vp]),
     "fuelgpu_global_tour_batch": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp]),
     "fuelgpu_global_tour_batch_dev": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp]),
+    "fuelgpu_kino_search_batch": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp, C.POINTER(FuelKinoParams), _vp, _vp, _vp,
+                                            _vp, _i32, _vp, _vp]),
+    "fuelgpu_kino_search_batch_dev": (C.c_int, [_vp, _i32, _vp, _vp, _vp, _vp, _vp, C.POINTER(FuelKinoParams), _vp,
+                                                _vp, _vp, _vp, _i32, _vp, _vp]),
 }
 
 _lib = None

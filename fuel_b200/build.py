@@ -9,10 +9,10 @@ CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libfuelgpu.so")
 SOURCES = ["api.cu", "esdf.cu", "esdf_tile.cu", "sharded.cu", "frontier.cu", "bspline.cu", "bspline_solve.cu", "bspline_solve_long.cu",
            "fusion.cu", "viewpoints.cu", "traj_check.cu", "poly_traj.cu", "astar.cu",
-           "view_cost.cu", "local_tour.cu", "global_tour.cu"]
+           "view_cost.cu", "local_tour.cu", "global_tour.cu", "kino_astar.cu"]
 FMAD_OK = {"bspline_solve.cu", "bspline_solve_long.cu", "esdf.cu", "esdf_tile.cu", "sharded.cu"}  # files whose arithmetic need not follow the host rounding sequence
 HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "bspline_eval.cuh"), os.path.join(CSRC, "raycast.cuh"),
-           os.path.join(CSRC, "heap.cuh"), os.path.join(ROOT, "include", "fuelgpu.h")]
+           os.path.join(CSRC, "heap.cuh"), os.path.join(CSRC, "kino_math.cuh"), os.path.join(ROOT, "include", "fuelgpu.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

@@ -275,6 +275,7 @@ int fuelgpu_map_destroy(FuelMap* m) {
   m->fr_scr.release();
   m->tc_buf.release();
   m->as_buf.release();
+  m->ks_buf.release();
   m->vc_buf.release();
   m->lt_buf.release();
   m->gt_buf.release();
@@ -1306,6 +1307,60 @@ int fuelgpu_astar_batch(FuelMap* m, int32_t B, const double* start, const double
   rc = st.upload();
   if (rc) return rc;
   rc = astar_impl(m, B, d_s, d_g, p, d_info, path_max, d_path, w_max, d_n, d_wp);
+  if (rc) return rc;
+  return st.download();
+}
+
+static int check_kino_args(FuelMap* m, int32_t B, const void* start, const void* vel, const void* acc, const void* goal,
+                           const FuelKinoParams* p, const void* info, const void* points, const void* derivs,
+                           const void* dt, int32_t node_max, const void* nodes) {
+  if (!m) return fuel_fail(nullptr, FUELGPU_EINVAL, "null map");
+  if (B < 0) return fuel_fail(m, FUELGPU_EINVAL, "negative batch");
+  const int rc = kino_check_params(m, p);
+  if (rc) return rc;
+  if (nodes && node_max < 1) return fuel_fail(m, FUELGPU_EINVAL, "node_max must be at least 1 with a node buffer");
+  if (B > 0 && (!start || !vel || !acc || !goal || !info || !points || !derivs || !dt))
+    return fuel_fail(m, FUELGPU_EINVAL, "null argument");
+  return 0;
+}
+
+int fuelgpu_kino_search_batch_dev(FuelMap* m, int32_t B, const void* start_dev, const void* vel_dev, const void* acc_dev,
+                                  const void* goal_dev, const void* gate_dev, const FuelKinoParams* p, void* info_dev,
+                                  void* points_dev, void* derivs_dev, void* dt_dev, int32_t node_max, void* nodes_dev,
+                                  void* shot_dev) {
+  int rc = check_kino_args(m, B, start_dev, vel_dev, acc_dev, goal_dev, p, info_dev, points_dev, derivs_dev, dt_dev,
+                           node_max, nodes_dev);
+  if (rc) return rc;
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  return kino_search_impl(m, B, (const double*)start_dev, (const double*)vel_dev, (const double*)acc_dev,
+                          (const double*)goal_dev, (const FuelPathInfo*)gate_dev, p, (FuelKinoInfo*)info_dev,
+                          (double*)points_dev, (double*)derivs_dev, (double*)dt_dev, node_max, (double*)nodes_dev,
+                          (double*)shot_dev);
+}
+
+int fuelgpu_kino_search_batch(FuelMap* m, int32_t B, const double* start, const double* vel, const double* acc,
+                              const double* goal, const FuelKinoParams* p, FuelKinoInfo* info, double* points,
+                              double* derivs, double* dt, int32_t node_max, double* nodes, double* shot) {
+  int rc = check_kino_args(m, B, start, vel, acc, goal, p, info, points, derivs, dt, node_max, nodes);
+  if (rc) return rc;
+  for (int32_t b = 0; b < B; ++b)
+    for (int k = 0; k < 3; ++k) {
+      const size_t i = 3 * (size_t)b + k;
+      if (!isfinite(start[i]) || !isfinite(vel[i]) || !isfinite(acc[i]) || !isfinite(goal[i]))
+        return fuel_fail(m, FUELGPU_EINVAL, "query %s%lld: start, vel, acc and goal must be finite", "", (long long)b);
+    }
+  if (B == 0) return 0;
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  const size_t nb = (size_t)B;
+  double *d_s, *d_v, *d_a, *d_g, *d_pts, *d_der, *d_dt, *d_nodes, *d_shot;
+  FuelKinoInfo* d_info;
+  HostStaging st(m);
+  st.in(&d_s, start, nb * 3).in(&d_v, vel, nb * 3).in(&d_a, acc, nb * 3).in(&d_g, goal, nb * 3).out(&d_info, info, nb);
+  st.out(&d_pts, points, nb * (FUELGPU_MAX_PTS - 2) * 3).out(&d_der, derivs, nb * 12).out(&d_dt, dt, nb);
+  st.out(&d_nodes, nodes, nodes ? nb * node_max * 12 : 0).out(&d_shot, shot, nb * 12);
+  rc = st.upload();
+  if (rc) return rc;
+  rc = kino_search_impl(m, B, d_s, d_v, d_a, d_g, nullptr, p, d_info, d_pts, d_der, d_dt, node_max, d_nodes, d_shot);
   if (rc) return rc;
   return st.download();
 }

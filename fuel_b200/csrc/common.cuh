@@ -93,6 +93,8 @@ struct FuelMap {
   DevBuf<uint8_t> lt_buf;  // local tour: the graph, its edges and their costs, the search state, the tour segments
   DevBuf<uint8_t> gt_buf;  // global tour: the instance table and the Held-Karp tables of one group (global_tour.cu)
   size_t as_stride, as_warps;  // layout whose key tables are known empty: per-warp bytes, warps
+  DevBuf<uint8_t> ks_buf;      // kinodynamic search scratch (kino_astar.cu)
+  size_t ks_stride, ks_warps;  // its layout whose key tables are known empty
 #ifdef FUEL_PROF
   double end_prof_us[3];  // the last fuelgpu_frontier_search_end: stream wait, result assembly, closing event (host µs)
 #endif
@@ -245,6 +247,11 @@ int astar_impl(FuelMap* m, int B, const double* start_dev, const double* goal_de
 int astar_raw_impl(FuelMap* m, int P, const int* n_list_dev, const int* list_dev, const double* p1_dev,
                    const double* p2_dev, const FuelAstarParams* p, FuelPathInfo* info_dev, int path_max,
                    double* path_dev);
+// kino_astar.cu: kinodynamicReplan's search, retry and getSamples (planner_manager.cpp:131-164) for B queries
+int kino_check_params(FuelMap* m, const FuelKinoParams* p);
+int kino_search_impl(FuelMap* m, int B, const double* start, const double* vel, const double* acc, const double* goal,
+                     const FuelPathInfo* gate, const FuelKinoParams* p, FuelKinoInfo* info, double* points,
+                     double* derivs, double* dt, int node_max, double* nodes, double* shot);
 // view_cost.cu: ViewNode::searchPath + computeCost (graph_node.cpp:32-85) for P pairs
 int view_cost_impl(FuelMap* m, int P, const double* p1, const double* p2, const double* y1, const double* y2,
                    const double* v1, const FuelViewCostParams* vp, FuelViewCostInfo* info_dev, int path_max,

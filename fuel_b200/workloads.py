@@ -542,3 +542,19 @@ def make_global_tours(n, B=1, seed=20261020, kind="geometric", vm=2.0, yd=60 * 3
         np.fill_diagonal(m, 0.0)
         out[b] = m
     return out
+
+
+def make_kino_queries(g, inflate, tri, info, start, goal, seed=20261019, max_vel=2.0, max_acc=2.0):
+    """kinodynamicReplan queries from the MID rows of a path search (info: FuelPathInfo rows of fuelgpu_astar_batch for
+    start / goal): start, goal and a start velocity and acceleration within the search's limits, as the exploration
+    FSM hands over the current state.  Returns dict(rows, start, vel, acc, goal) with rows the MID indices."""
+    rng = np.random.default_rng(seed)
+    rows = np.flatnonzero((info["status"] == 1) & (info["branch"] == 2))
+    n = len(rows)
+    vel = rng.uniform(-1, 1, (n, 3)) * max_vel * 0.6
+    vel[:, 2] *= 0.3
+    acc = rng.uniform(-1, 1, (n, 3)) * max_acc * 0.5
+    still = rng.random(n) < 0.2  # hovering before the replan
+    vel[still] = 0.0
+    acc[still] = 0.0
+    return dict(rows=rows, start=np.asarray(start)[rows].copy(), vel=vel, acc=acc, goal=np.asarray(goal)[rows].copy())

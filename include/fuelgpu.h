@@ -601,7 +601,7 @@ FUELGPU_API int fuelgpu_yaw_explore_batch_dev(FuelMap* map, int32_t B, int32_t n
  * planExploreTraj a single point -- or one longer than FUELGPU_MAX_WAYPTS or w_max); the poly entry's _dev form marks
  * an n_wp of 0 FUELGPU_POLY_BAD_INPUT and leaves the other rows alone, so fuelgpu_astar_batch_dev ->
  * fuelgpu_poly_waypoints_batch_dev -> ... needs no host sync.  A MID tour (1.5 <= length <= 5.0) is written too: the
- * reference calls kinodynamicReplan there instead, which this library does not replace, so the caller decides.
+ * reference calls kinodynamicReplan there instead, which fuelgpu_kino_search_batch_dev runs on exactly these rows.
  * Scratch: one map-owned device buffer, grown on demand: W warps search at once, W = min(B, 32 * SM count,
  * max(1, 4 GiB / S)), with S = 80 * allocate_num + 16 * T + 24 bytes per warp (each array rounded up to 256 bytes), T the
  * least power of two >= max(64, 2 * allocate_num), and 256 bytes more; FUELGPU_ENOMEM if it cannot be allocated.  Runs on the map's main stream;
@@ -620,7 +620,8 @@ FUELGPU_API int fuelgpu_yaw_explore_batch_dev(FuelMap* map, int32_t B, int32_t n
 /* FuelPathInfo.branch (fast_exploration_manager.cpp:243-275) */
 #define FUELGPU_ASTAR_NONE 0
 #define FUELGPU_ASTAR_CLOSE 1 /* length < 1.5: the whole tour, next_goal = goal */
-#define FUELGPU_ASTAR_MID 2   /* otherwise: the reference runs kinodynamicReplan; the whole tour, next_goal = goal */
+#define FUELGPU_ASTAR_MID 2   /* otherwise: the reference runs kinodynamicReplan (fuelgpu_kino_search_batch_dev); the
+                                 whole tour, next_goal = goal */
 #define FUELGPU_ASTAR_FAR 3   /* length > 5.0: the tour truncated past 5 m, next_goal = its last point */
 /* FuelPathInfo.tour_status */
 #define FUELGPU_ASTAR_TOO_LONG 1   /* more than FUELGPU_MAX_WAYPTS or w_max points */
@@ -648,6 +649,81 @@ FUELGPU_API int fuelgpu_astar_batch(FuelMap* map, int32_t B, const double* start
 FUELGPU_API int fuelgpu_astar_batch_dev(FuelMap* map, int32_t B, const void* start_dev, const void* goal_dev,
                                         const FuelAstarParams* params, void* info_dev, int32_t path_max, void* path_dev,
                                         int32_t w_max, void* n_wp_dev, void* waypts_dev);
+
+/* ---- kinodynamic path to a mid-range goal: kinodynamicReplan's search on the device --------------------------------
+ * Replaces, for B queries, FastPlannerManager::kinodynamicReplan(start, vel, acc, goal, 0, time_lb) up to its
+ * parameterization (plan_manage/src/planner_manager.cpp:131-164): the "Close goal" refusal (|start - goal| < 1e-2),
+ * KinodynamicAstar::reset and the non-dynamic search(start, vel, acc, goal, 0, init = true) with the retry at
+ * init = false after NO_PATH (path_searching/src/kinodynamic_astar.cpp:15-263), computeShotTraj and getSamples at
+ * ts = ctrl_pt_dist / manager_max_vel, laid out as the input of fuelgpu_bspline_parameterize_batch[_dev] (with the
+ * caller's time_lb).  Every search reads the resident occupancy byte with the reference's tests: isInBox, the inflate bit,
+ * UNKNOWN unless optimistic; the shot's samples are bounded by origin below and by the map's SIZE above (the reference's
+ * getRegion) and tested against the inflate bit alone.  Nodes are keyed by floor((p - origin) / resolution) on the map's
+ * origin; the open set is libstdc++'s std::priority_queue restated over node ids, compared through each node's current
+ * f_score.  Arithmetic (DESIGN.md 4.14): the search's powers are host tables of 0.5 * pow(t, 2) computed with the host's
+ * pow in the reference's loops, and cbrt is glibc's routine restated, so the search equals the reference's glibc build
+ * bit for bit except where cubic()'s three-real-root branch (D < 0) runs: there acos and cos are correctly rounded.  Outside
+ * the search (the shot and getSamples) pow(t, 2) and pow(t, 3) are correctly rounded.
+ *   start, vel, acc, goal [B][3]   finite; end_v is 0, as planExploreMotion passes it
+ *   params                        the search/ parameters (max_vel without vel_margin: the search adds it), ctrl_pt_dist and
+ *                                 manager_max_vel (pp_.max_vel_).  The duration and acceleration lists follow the
+ *                                 reference's loops; at most 32 init durations and 8 steps per axis (the loop of
+ *                                 the other durations always yields max_tau alone).
+ * Outputs: info [B]; points [B][FUELGPU_MAX_PTS-2][3] (the K = n_pts - 2 samples of getSamples, rows >= K zero); derivs
+ * [B][4][3] (start vel, end vel, start acc, end acc); dt [B] (getSamples' ts; NaN without samples, so that
+ * fuelgpu_bspline_parameterize_batch_dev marks the row); nodes [B][node_max][12] or NULL (state, input, duration, g, f of
+ * the path root .. end node; the root's input and duration 0); shot [B][3][4] or NULL (coef_shot_, zero without a shot).
+ * A path of more than FUELGPU_MAX_PTS - 2 samples gets traj_status FUELGPU_KINO_TOO_LONG and no samples.
+ * The _dev entry takes gate, the info of fuelgpu_astar_batch_dev, or NULL: rows whose branch is not FUELGPU_ASTAR_MID get
+ * status FUELGPU_KINO_SKIPPED, so astar_batch_dev -> kino_search_batch_dev -> parameterize_batch_dev needs no host sync
+ * except to read info[].n_pts.  A node pool of allocate_num per search; use_node_num_ reaching it ends the search with
+ * NO_PATH, reason FUELGPU_KINO_POOL.
+ * Scratch: one map-owned device buffer, grown on demand: W warps search at once, W = min(B, 32 * SM count,
+ * max(1, 4 GiB / S)), S about 153 * allocate_num + 56 KiB per warp; FUELGPU_ENOMEM if it cannot be allocated.  Runs on the
+ * map's main stream; not timed in fuelgpu_map_last_timing.  The host entry returns FUELGPU_EINVAL and writes nothing on a
+ * non-finite input or a bad parameter; the _dev entry checks the parameters alone and marks a row with a non-finite input
+ * FUELGPU_KINO_BAD_INPUT, leaving the other rows unaffected. */
+/* FuelKinoInfo.status: KinodynamicAstar's codes for the attempt that counted, then the rows not searched */
+#define FUELGPU_KINO_REACH_HORIZON 1
+#define FUELGPU_KINO_REACH_END 2
+#define FUELGPU_KINO_NO_PATH 3
+#define FUELGPU_KINO_NEAR_END 4
+#define FUELGPU_KINO_SKIPPED 5   /* _dev with gate: not a MID row */
+#define FUELGPU_KINO_BAD_INPUT 6 /* _dev only: a non-finite start, vel, acc or goal */
+/* FuelKinoInfo.reason */
+#define FUELGPU_KINO_FOUND 0
+#define FUELGPU_KINO_OPEN_EMPTY 1     /* the open set ran empty (:259-262) */
+#define FUELGPU_KINO_POOL 2           /* use_node_num_ == allocate_num_ right after an allocation (:235-239) */
+#define FUELGPU_KINO_START_NEAR_END 3 /* the start node lies within the goal tolerance and has no shot (:90-93) */
+#define FUELGPU_KINO_CLOSE_GOAL 4     /* |start - goal| < 1e-2: kinodynamicReplan returns before searching */
+/* FuelKinoInfo.traj_status */
+#define FUELGPU_KINO_TOO_LONG 1 /* more than FUELGPU_MAX_PTS - 2 samples */
+#define FUELGPU_KINO_NO_TRAJ 2  /* no samples: NO_PATH, skipped or bad input */
+typedef struct {
+  double max_tau, init_max_tau; /* search/max_tau, search/init_max_tau */
+  double max_vel, vel_margin;   /* search/max_vel, search/vel_margin: the search's max_vel_ is their sum */
+  double max_acc, w_time, horizon, lambda_heu;
+  double resolution;            /* search/resolution_astar */
+  double ctrl_pt_dist;          /* manager/control_points_distance */
+  double manager_max_vel;       /* manager/max_vel: ts = ctrl_pt_dist / manager_max_vel */
+  int32_t allocate_num, check_num, optimistic, reserved;
+} FuelKinoParams;
+typedef struct {
+  int32_t status, reason, retried, traj_status; /* retried: the init = false search ran */
+  int32_t iter_num, use_node_num;               /* iter_num_, use_node_num_ after the attempt that counted */
+  int32_t n_nodes, shot;                        /* path_nodes_.size(), is_shot_succ_ */
+  int32_t seg_num, n_pts;                       /* getSamples' seg_num; n_pts = K + 2 (0 without samples) */
+  double t_shot, T_sum;
+} FuelKinoInfo;
+FUELGPU_API int fuelgpu_kino_search_batch(FuelMap* map, int32_t B, const double* start, const double* vel,
+                                          const double* acc, const double* goal, const FuelKinoParams* params,
+                                          FuelKinoInfo* info, double* points, double* derivs, double* dt,
+                                          int32_t node_max, double* nodes, double* shot);
+FUELGPU_API int fuelgpu_kino_search_batch_dev(FuelMap* map, int32_t B, const void* start_dev, const void* vel_dev,
+                                              const void* acc_dev, const void* goal_dev, const void* gate_dev,
+                                              const FuelKinoParams* params, void* info_dev, void* points_dev,
+                                              void* derivs_dev, void* dt_dev, int32_t node_max, void* nodes_dev,
+                                              void* shot_dev);
 
 /* ---- tour cost between viewpoints: ViewNode::searchPath and ViewNode::computeCost on the device -------------------
  * For P pairs (p1, p2, y1, y2, v1), what ViewNode::computeCost(p1, p2, y1, y2, v1, 0, path)

@@ -367,6 +367,51 @@ private:
   int allocate_num_ = 100000, use_node_num_ = 0, iter_num_ = 0;
 };
 
+// ---- KinodynamicAstar (path_searching/include/path_searching/kinodynamic_astar.h) over fuelgpu_kino_search_batch ------
+// What FastPlannerManager::kinodynamicReplan (planner_manager.cpp:131-164) does with kino_path_finder_, on the device of
+// the environment's map: search() runs the close-goal refusal, search(init = true) and, after NO_PATH, reset and
+// search(init = false), and returns the status of the attempt that counted; getSamples() returns the samples at
+// ts = ctrl_pt_dist / manager_max_vel.  setParam() takes the search/ parameters as FuelKinoParams.
+class KinodynamicAstar {
+public:
+  enum { REACH_HORIZON = 1, REACH_END = 2, NO_PATH = 3, NEAR_END = 4 };
+  void setParam(const FuelKinoParams& p) { p_ = p; }
+  void setEnvironment(const EDTEnvironment::Ptr& env) { edt_env_ = env; }
+  void init() {}
+  void reset() {
+    info_ = FuelKinoInfo();
+    points_.clear();
+  }
+  int search(const Vector3d& start_pt, const Vector3d& start_vel, const Vector3d& start_acc, const Vector3d& end_pt) {
+    FuelMap* h = edt_env_->sdf_map_->gpu();
+    const double s[3] = { start_pt(0), start_pt(1), start_pt(2) }, v[3] = { start_vel(0), start_vel(1), start_vel(2) };
+    const double a[3] = { start_acc(0), start_acc(1), start_acc(2) }, e[3] = { end_pt(0), end_pt(1), end_pt(2) };
+    double pts[3 * (FUELGPU_MAX_PTS - 2)], der[12], shot[12];
+    fuelgpu_check(fuelgpu_kino_search_batch(h, 1, s, v, a, e, &p_, &info_, pts, der, &ts_, 0, nullptr, shot), h);
+    points_.clear();
+    for (int i = 0; i + 2 < info_.n_pts; ++i) points_.push_back(Vector3d(pts[3 * i], pts[3 * i + 1], pts[3 * i + 2]));
+    derivs_.clear();
+    for (int i = 0; i < 4; ++i) derivs_.push_back(Vector3d(der[3 * i], der[3 * i + 1], der[3 * i + 2]));
+    return info_.status;
+  }
+  // false when the search left no samples (NO_PATH or more than FUELGPU_MAX_PTS - 2 of them)
+  bool getSamples(double& ts, std::vector<Vector3d>& point_set, std::vector<Vector3d>& start_end_derivatives) const {
+    if (info_.traj_status != 0) return false;
+    ts = ts_;
+    point_set = points_;
+    start_end_derivatives = derivs_;
+    return true;
+  }
+  const FuelKinoInfo& info() const { return info_; }
+
+private:
+  EDTEnvironment::Ptr edt_env_;
+  FuelKinoParams p_{ 0.8, 1.0, 2.0, 0.25, 2.0, 10.0, 5.0, 10.0, 0.025, 0.35, 2.0, 100000, 10, 0, 0 };  // algorithm.xml
+  FuelKinoInfo info_{};
+  double ts_ = 0.0;
+  std::vector<Vector3d> points_, derivs_;
+};
+
 // ---- ViewNode (graph_node.h:49-84) over fuelgpu_view_cost_batch ------------------------------------------------
 // Set the statics as FastExplorationManager::initialize does (fast_exploration_manager.cpp:55-69): vm_, yd_, w_dir_ from
 // exploration/*, astar_param_ from astar/* (max_iter standing for max_search_time_; searchPath searches at resolution
