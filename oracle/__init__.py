@@ -12,7 +12,6 @@ import subprocess
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "libfuel_oracle.so")
 
 ORC_MAX_PTS = 64
 
@@ -23,18 +22,41 @@ NORMAL_PHASE = SMOOTHNESS | DISTANCE | FEASIBILITY | START | END
 GUIDE_PHASE = SMOOTHNESS | GUIDE | START | END
 
 
-def build(force=False):
-    """Compile the oracle with the committed Makefile (gcc -O3, the reference's flags)."""
-    src = [os.path.join(_HERE, f) for f in ("fuel_oracle.c", "fuel_oracle_fusion.c", "fuel_oracle_viewpoints.c",
-                                            "fuel_oracle.h", "Makefile", "ref_raycast_wrap.cpp", "ref_sdfmap_wrap.cpp", "ref_bspline_wrap.cpp",
-                                            "ref_frontier_wrap.cpp")]
-    ref_src = "/root/reference/fuel_planner/plan_env/src/raycast.cpp"
-    ref_ok = not os.path.exists(ref_src) or os.path.exists(os.path.join(_HERE, "_ref", "libfuel_ref.so"))
-    if (not force and os.path.exists(_SO) and ref_ok
-            and all(os.path.getmtime(_SO) >= os.path.getmtime(s) for s in src)):
-        return _SO
-    subprocess.check_call(["make", "-C", _HERE, "-s"])
-    return _SO
+# The oracle's parts in build order, each a module with its own build().
+PARTS = ("oracle", "oracle.traj", "oracle.param", "oracle.poly", "oracle.yaw", "oracle.astar", "oracle.view",
+         "oracle.tour", "oracle.gtour", "oracle.kino")
+
+
+def _make(mk=None):
+    """make -s -C oracle [-f mk]: each recipe declares what its libraries are built from, so make rebuilds whatever is
+    stale, and builds the reference's side only where the reference's sources are present."""
+    subprocess.check_call(["make", "-s", "-C", _HERE] + (["-f", mk] if mk else []))
+
+
+_loaded = {}
+
+
+def _load(name, restypes, build=None, first=None):
+    """oracle/<name>, loaded once with the restypes of `restypes` ({symbol: ctypes type}) set.  A part's own library
+    (`build` given) is built first.  A reference library is None where it is not built, or where `first()` is None:
+    `first` loads, before this library, the one whose symbols it binds to or whose objects its callers hand it."""
+    L = _loaded.get(name)
+    if L is None:
+        path = os.path.join(_HERE, name)
+        if build is not None:
+            build()
+        elif not os.path.exists(path) or (first is not None and first() is None):
+            return None
+        L = _loaded[name] = C.CDLL(path)
+        for sym, ty in restypes.items():
+            getattr(L, sym).restype = ty
+    return L
+
+
+def build():
+    """Compile the oracle with the committed Makefile (gcc -O3, the reference's flags), and _ref/libfuel_ref.so where
+    the reference's sources are present."""
+    _make()
 
 
 class OrcGrid(C.Structure):
@@ -90,21 +112,13 @@ class OrcSolveParams(C.Structure):
     _fields_ = [("max_eval", C.c_int32), ("lbfgs_m", C.c_int32), ("xtol_rel", C.c_double)]
 
 
-_lib = None
-
-
 def lib():
-    global _lib
-    if _lib is None:
-        build()
-        _lib = C.CDLL(_SO)
-        _lib.orc_dist_with_grad.restype = C.c_double
-        _lib.orc_pt_dist.restype = C.c_double
-        _lib.orc_frontier_search.restype = C.c_void_p
-        for name in ("orc_frontier_count", "orc_frontier_num_cells", "orc_frontier_num_filtered",
-                     "orc_frontier_is_changed", "orc_is_frontier_cell", "orc_is_in_map_pos"):
-            getattr(_lib, name).restype = C.c_int32
-    return _lib
+    i32 = C.c_int32
+    return _load("libfuel_oracle.so", dict(orc_dist_with_grad=C.c_double, orc_pt_dist=C.c_double,
+                                           orc_frontier_search=C.c_void_p, orc_frontier_count=i32,
+                                           orc_frontier_num_cells=i32, orc_frontier_num_filtered=i32,
+                                           orc_frontier_is_changed=i32, orc_is_frontier_cell=i32, orc_is_in_map_pos=i32),
+                 build=build)
 
 
 def _p(a, ty=None):
@@ -294,20 +308,13 @@ def raycast_ids(g, start, end, max_ids=8192):
     return out[:n]
 
 
-_REF_RAYCAST = os.path.join(_HERE, "_ref", "libfuel_ref.so")
-_ref_rc = None
-
-
 def ref_raycast():
     """The REFERENCE's own code (plan_env/src/raycast.cpp + sdf_map.cpp compiled unmodified into
-    oracle/_ref/libfuel_ref.so by the Makefile, only where /root/reference exists) or None."""
-    global _ref_rc
-    if _ref_rc is None and os.path.exists(_REF_RAYCAST):
-        _ref_rc = C.CDLL(_REF_RAYCAST)
-        _ref_rc.ref_raycast_ids.restype = C.c_int32
-        _ref_rc.ref_intbound.restype = C.c_double
-        _ref_rc.ref_intbound.argtypes = [C.c_double, C.c_double]
-    return _ref_rc
+    oracle/_ref/libfuel_ref.so by the Makefile, only where the reference's sources are present) or None."""
+    R = _load("_ref/libfuel_ref.so", dict(ref_raycast_ids=C.c_int32, ref_intbound=C.c_double))
+    if R is not None:
+        R.ref_intbound.argtypes = [C.c_double, C.c_double]
+    return R
 
 
 def ref_raycast_ids(g, start, end, max_ids=8192):

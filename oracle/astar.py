@@ -5,17 +5,10 @@ branch) and of the reference's own path_searching/src/astar2.cpp run through ora
 TEST INFRASTRUCTURE ONLY, like the rest of this package: fuel_b200/ must never import it.
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from . import _p
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "libfuel_oracle_astar.so")
-_REF_SO = os.path.join(_HERE, "_ref", "libfuel_ref_astar.so")
-_REF_SRC = "/root/reference/fuel_planner/path_searching/src/astar2.cpp"
+from . import _load, _make, _p, ref_raycast
 
 # the layout of FuelPathInfo (include/fuelgpu.h)
 INFO_DTYPE = np.dtype([("status", np.int32), ("reason", np.int32), ("iter_num", np.int32), ("use_node_num", np.int32),
@@ -28,39 +21,19 @@ class OrcAstarMap(C.Structure):
                 ("box_mind", C.c_double * 3), ("box_maxd", C.c_double * 3), ("occ", C.c_void_p)]
 
 
-def build(force=False):
+def build():
     """Compile this part with oracle/astar.mk."""
-    src = [os.path.join(_HERE, f) for f in ("fuel_oracle_astar.c", "fuel_oracle_astar.h", "astar.mk", "ref_astar_wrap.cpp")]
-    ref_ok = not os.path.exists(_REF_SRC) or os.path.exists(_REF_SO)
-    if (not force and os.path.exists(_SO) and ref_ok
-            and all(os.path.getmtime(_SO) >= os.path.getmtime(s) for s in src if os.path.exists(s))):
-        return _SO
-    subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "astar.mk"])
-    return _SO
-
-
-_lib = None
-_ref = None
+    _make("astar.mk")
 
 
 def lib():
-    global _lib
-    if _lib is None:
-        build()
-        _lib = C.CDLL(_SO)
-        _lib.orc_astar.restype = C.c_int32
-    return _lib
+    return _load("libfuel_oracle_astar.so", dict(orc_astar=C.c_int32), build=build)
 
 
 def ref_astar():
-    """The REFERENCE's astar2.cpp + oracle/ref_astar_wrap.cpp, or None where it is not built."""
-    global _ref
-    if _ref is None and os.path.exists(_REF_SO):
-        from . import ref_raycast
-        ref_raycast()  # libfuel_ref.so (SDFMap, RayCaster) first
-        _ref = C.CDLL(_REF_SO)
-        _ref.ref_astar_create.restype = C.c_void_p
-    return _ref
+    """The REFERENCE's astar2.cpp + oracle/ref_astar_wrap.cpp over libfuel_ref.so's SDFMap and RayCaster, or None where
+    it is not built."""
+    return _load("_ref/libfuel_ref_astar.so", dict(ref_astar_create=C.c_void_p), first=ref_raycast)
 
 
 def occ_byte(inflate, tri):

@@ -6,17 +6,10 @@ library where the reference's sources are present.  The map is the reference's S
 TEST INFRASTRUCTURE ONLY, like the rest of this package: fuel_b200/ must never import it.
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from . import _p
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "libfuel_oracle_gtour.so")
-_REF_SO = os.path.join(_HERE, "_ref", "libfuel_ref_gtour.so")
-_REF_SRC = "/root/reference/fuel_planner/utils/lkh_tsp_solver/src/lkh_interface.cpp"
+from . import _load, _make, _p, ref_raycast
 
 GTOUR_OK, GTOUR_BAD_INPUT, GTOUR_TOO_LARGE = 0, 1, 2
 GTOUR_MAX_CLUSTERS = 20
@@ -25,28 +18,13 @@ GTOUR_DTYPE = np.dtype([("status", np.int32), ("n", np.int32), ("n_optimal", np.
                         ("cost", np.int64)])
 
 
-def build(force=False):
+def build():
     """Compile this part with oracle/gtour.mk."""
-    src = [os.path.join(_HERE, f) for f in ("fuel_oracle_gtour.c", "fuel_oracle_gtour.h", "gtour.mk",
-                                            "ref_gtour_wrap.cpp")]
-    ref_ok = not os.path.exists(_REF_SRC) or os.path.exists(_REF_SO)
-    if (not force and os.path.exists(_SO) and ref_ok
-            and all(os.path.getmtime(_SO) >= os.path.getmtime(s) for s in src if os.path.exists(s))):
-        return _SO
-    subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "gtour.mk"])
-    return _SO
-
-
-_lib = None
+    _make("gtour.mk")
 
 
 def lib():
-    global _lib
-    if _lib is None:
-        build()
-        _lib = C.CDLL(_SO)
-        _lib.orc_global_tour.restype = C.c_int32
-    return _lib
+    return _load("libfuel_oracle_gtour.so", dict(orc_global_tour=C.c_int32), build=build)
 
 
 def int_matrix(mat):
@@ -96,20 +74,11 @@ def global_tour_batch(dims, cost):
     return info, indices
 
 
-_ref_gtour = None
-
-
 def ref_gtour():
-    """The REFERENCE's fast_exploration_manager.cpp + frontier_finder.cpp + LKH + oracle/ref_gtour_wrap.cpp, or None
-    where it is not built."""
-    global _ref_gtour
-    if _ref_gtour is None and os.path.exists(_REF_SO):
-        from . import ref_raycast
-        ref_raycast()  # libfuel_ref.so (SDFMap, RayCaster) first
-        _ref_gtour = C.CDLL(_REF_SO)
-        for f in ("ref_gtour_setup", "ref_gtour_find"):
-            getattr(_ref_gtour, f).restype = C.c_int32
-    return _ref_gtour
+    """The REFERENCE's fast_exploration_manager.cpp + frontier_finder.cpp + LKH + oracle/ref_gtour_wrap.cpp over
+    libfuel_ref.so's SDFMap and RayCaster, or None where it is not built."""
+    return _load("_ref/libfuel_ref_gtour.so", dict(ref_gtour_setup=C.c_int32, ref_gtour_find=C.c_int32),
+                 first=ref_raycast)
 
 
 def _f64(a, shape=(-1,)):

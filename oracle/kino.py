@@ -5,20 +5,10 @@ getSamples, in the reference's glibc arithmetic or in the device's) and of the h
 TEST INFRASTRUCTURE ONLY, like the rest of this package: fuel_b200/ must never import it.
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from . import _p
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "libfuel_oracle_kino.so")
-_REF_SO = os.path.join(_HERE, "_ref", "libfuel_ref_kino.so")
-_REF_SRC = "/root/reference/fuel_planner/path_searching/src/kinodynamic_astar.cpp"
-_SRC = [os.path.join(_HERE, f) for f in ("fuel_oracle_kino.c", "fuel_oracle_kino.h", "kino_math_host.cpp", "kino.mk",
-                                         "ref_kino_wrap.cpp")] + \
-       [os.path.join(os.path.dirname(_HERE), "fuel_b200", "csrc", "kino_math.cuh")]
+from . import _load, _make, _p, ref_raycast
 GLIBC, DEVICE = 0, 1
 MAX_PTS = 64
 
@@ -30,27 +20,14 @@ INFO_DTYPE = np.dtype([("status", np.int32), ("reason", np.int32), ("retried", n
 MATH_CBRT, MATH_CUBE, MATH_ACOS, MATH_COS, MATH_LIBM_CBRT = 0, 1, 2, 3, 4
 
 
-def build(force=False):
+def build():
     """Compile this part with oracle/kino.mk."""
-    ref_ok = not os.path.exists(_REF_SRC) or os.path.exists(_REF_SO)
-    if not force and os.path.exists(_SO) and ref_ok and all(os.path.getmtime(_SO) >= os.path.getmtime(s) for s in _SRC):
-        return _SO
-    subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "kino.mk"])
-    return _SO
-
-
-_lib = None
-_ref = None
+    _make("kino.mk")
 
 
 def lib():
-    global _lib
-    if _lib is None:
-        build()
-        _lib = C.CDLL(_SO)
-        _lib.orc_kino_replan.restype = C.c_int32
-        _lib.orc_kino_three_root_count.restype = C.c_longlong
-    return _lib
+    return _load("libfuel_oracle_kino.so", dict(orc_kino_replan=C.c_int32, orc_kino_three_root_count=C.c_longlong),
+                 build=build)
 
 
 def three_root_count(reset=True):
@@ -59,14 +36,9 @@ def three_root_count(reset=True):
 
 
 def ref_kino():
-    """The REFERENCE's kinodynamic_astar.cpp + oracle/ref_kino_wrap.cpp, or None where it is not built."""
-    global _ref
-    if _ref is None and os.path.exists(_REF_SO):
-        from . import ref_raycast
-        ref_raycast()  # libfuel_ref.so (SDFMap) first
-        _ref = C.CDLL(_REF_SO)
-        _ref.ref_kino_create.restype = C.c_void_p
-    return _ref
+    """The REFERENCE's kinodynamic_astar.cpp + oracle/ref_kino_wrap.cpp over libfuel_ref.so's SDFMap, or None where it
+    is not built."""
+    return _load("_ref/libfuel_ref_kino.so", dict(ref_kino_create=C.c_void_p), first=ref_raycast)
 
 
 class RefKino:

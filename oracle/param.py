@@ -6,55 +6,27 @@ present).
 TEST INFRASTRUCTURE ONLY, like the rest of this package: fuel_b200/ must never import it.
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from . import OrcTrajConst, _p
+from . import OrcTrajConst, _load, _make, _p
 from . import traj as _traj
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "libfuel_oracle_param.so")
-_REF_SO = os.path.join(_HERE, "_ref", "libfuel_ref_param.so")
-_REF_SRC = "/root/reference/fuel_planner/bspline/src/non_uniform_bspline.cpp"
 
-
-def build(force=False):
+def build():
     """Compile the trajectory oracle first (oracle/traj.py), then this part with oracle/param.mk."""
     _traj.build()
-    src = [os.path.join(_HERE, f) for f in ("fuel_oracle_param.c", "fuel_oracle_param.h", "fuel_oracle_traj.h",
-                                            "fuel_oracle.h", "param.mk", "ref_param_wrap.cpp", "libfuel_oracle.so",
-                                            "libfuel_oracle_traj.so", os.path.join("ref_standin_param", "Eigen", "Eigen"))]
-    ref_ok = not os.path.exists(_REF_SRC) or os.path.exists(_REF_SO)
-    if (not force and os.path.exists(_SO) and ref_ok
-            and all(os.path.getmtime(_SO) >= os.path.getmtime(s) for s in src)):
-        return _SO
-    subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "param.mk"])
-    return _SO
-
-
-_lib = None
-_ref = None
+    _make("param.mk")
 
 
 def lib():
-    global _lib
-    if _lib is None:
-        build()
-        _lib = C.CDLL(_SO)
-        _lib.orc_lstsq_colpiv_qr.restype = C.c_int32
-    return _lib
+    return _load("libfuel_oracle_param.so", dict(orc_lstsq_colpiv_qr=C.c_int32), build=build)
 
 
 def ref_param():
-    """The REFERENCE's non_uniform_bspline.cpp + oracle/ref_param_wrap.cpp, or None where it is not built."""
-    global _ref
-    if _ref is None and os.path.exists(_REF_SO):
-        lib()  # the stand-in's solve binds to this library's orc_lstsq_colpiv_qr
-        _ref = C.CDLL(_REF_SO)
-        _ref.ref_param_parameterize.restype = C.c_int32
-    return _ref
+    """The REFERENCE's non_uniform_bspline.cpp + oracle/ref_param_wrap.cpp, or None where it is not built.  The
+    stand-in's solve binds to lib()'s orc_lstsq_colpiv_qr."""
+    return _load("_ref/libfuel_ref_param.so", dict(ref_param_parameterize=C.c_int32), first=lib)
 
 
 def param_system(points, derivs, ts):

@@ -5,55 +5,29 @@ getLength, planExploreTraj's sampling) and of the reference's own polynomial_tra
 TEST INFRASTRUCTURE ONLY, like the rest of this package: fuel_b200/ must never import it.
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from . import _p
+from . import _load, _make, _p
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "libfuel_oracle_poly.so")
-_REF_SO = os.path.join(_HERE, "_ref", "libfuel_ref_poly.so")
-_REF_SRC = "/root/reference/fuel_planner/poly_traj/src/polynomial_traj.cpp"
 MAX_K = 62  # FUELGPU_MAX_PTS - 2
 
 
-def build(force=False):
+def build():
     """Compile this part with oracle/poly.mk."""
-    src = [os.path.join(_HERE, f) for f in ("fuel_oracle_poly.c", "fuel_oracle_poly.h", "poly.mk", "ref_poly_wrap.cpp",
-                                            os.path.join("ref_standin_poly", "Eigen", "Eigen"))]
-    ref_ok = not os.path.exists(_REF_SRC) or os.path.exists(_REF_SO)
-    if (not force and os.path.exists(_SO) and ref_ok
-            and all(os.path.getmtime(_SO) >= os.path.getmtime(s) for s in src)):
-        return _SO
-    subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "poly.mk"])
-    return _SO
-
-
-_lib = None
-_ref = None
+    _make("poly.mk")
 
 
 def lib():
-    global _lib
-    if _lib is None:
-        build()
-        _lib = C.CDLL(_SO)
-        for f in ("orc_lu_inverse", "orc_poly_waypoints", "orc_explore_samples"):
-            getattr(_lib, f).restype = C.c_int32
-        _lib.orc_poly_total_time.restype = C.c_double
-        _lib.orc_poly_length.restype = C.c_double
-    return _lib
+    return _load("libfuel_oracle_poly.so", dict(orc_lu_inverse=C.c_int32, orc_poly_waypoints=C.c_int32,
+                                                orc_explore_samples=C.c_int32, orc_poly_total_time=C.c_double,
+                                                orc_poly_length=C.c_double), build=build)
 
 
 def ref_poly():
-    """The REFERENCE's polynomial_traj.cpp + oracle/ref_poly_wrap.cpp, or None where it is not built."""
-    global _ref
-    if _ref is None and os.path.exists(_REF_SO):
-        lib()  # the stand-in's inverse() binds to this library's orc_lu_inverse
-        _ref = C.CDLL(_REF_SO)
-    return _ref
+    """The REFERENCE's polynomial_traj.cpp + oracle/ref_poly_wrap.cpp, or None where it is not built.  The stand-in's
+    inverse() binds to lib()'s orc_lu_inverse."""
+    return _load("_ref/libfuel_ref_poly.so", {}, first=lib)
 
 
 def _v(a, n=None):

@@ -7,17 +7,10 @@ oracle/tour.mk, the reference library where the reference's sources are present.
 TEST INFRASTRUCTURE ONLY, like the rest of this package: fuel_b200/ must never import it.
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from . import _p
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "libfuel_oracle_tour.so")
-_REF_SO = os.path.join(_HERE, "_ref", "libfuel_ref_tour.so")
-_REF_SRC = "/root/reference/fuel_planner/exploration_manager/src/fast_exploration_manager.cpp"
+from . import _load, _make, _p, ref_raycast
 
 # the layout of FuelLocalTourInfo (include/fuelgpu.h)
 TOUR_DTYPE = np.dtype([("status", np.int32), ("n_nodes", np.int32), ("n_edges", np.int32), ("n_evals", np.int32),
@@ -25,29 +18,13 @@ TOUR_DTYPE = np.dtype([("status", np.int32), ("n_nodes", np.int32), ("n_edges", 
                        ("g", np.float64)])
 
 
-def build(force=False):
+def build():
     """Compile this part with oracle/tour.mk."""
-    src = [os.path.join(_HERE, f) for f in ("fuel_oracle_tour.c", "fuel_oracle_tour.h", "fuel_oracle_view.c",
-                                            "fuel_oracle_view.h", "fuel_oracle_astar.c", "fuel_oracle_astar.h",
-                                            "tour.mk", "ref_tour_wrap.cpp")]
-    ref_ok = not os.path.exists(_REF_SRC) or os.path.exists(_REF_SO)
-    if (not force and os.path.exists(_SO) and ref_ok
-            and all(os.path.getmtime(_SO) >= os.path.getmtime(s) for s in src if os.path.exists(s))):
-        return _SO
-    subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "tour.mk"])
-    return _SO
-
-
-_lib = None
+    _make("tour.mk")
 
 
 def lib():
-    global _lib
-    if _lib is None:
-        build()
-        _lib = C.CDLL(_SO)
-        _lib.orc_local_tour.restype = C.c_int32
-    return _lib
+    return _load("libfuel_oracle_tour.so", dict(orc_local_tour=C.c_int32), build=build)
 
 
 def edge_offsets(prob_off, group_off):
@@ -104,20 +81,11 @@ def local_tour_batch(m, prob_off, group_off, cur_pos, cur_vel, cur_yaw, vp_pos, 
     return info, refined, tour, edge_cost
 
 
-_ref_tour = None
-
-
 def ref_tour():
-    """The REFERENCE's fast_exploration_manager.cpp + frontier_finder.cpp + oracle/ref_tour_wrap.cpp, or None where it is
-    not built."""
-    global _ref_tour
-    if _ref_tour is None and os.path.exists(_REF_SO):
-        from . import ref_raycast
-        ref_raycast()  # libfuel_ref.so (SDFMap, RayCaster) first
-        _ref_tour = C.CDLL(_REF_SO)
-        for f in ("ref_tour_viewpoints", "ref_tour_select_ids", "ref_tour_pick"):
-            getattr(_ref_tour, f).restype = C.c_int32
-    return _ref_tour
+    """The REFERENCE's fast_exploration_manager.cpp + frontier_finder.cpp + oracle/ref_tour_wrap.cpp over libfuel_ref.so's
+    SDFMap and RayCaster, or None where it is not built."""
+    return _load("_ref/libfuel_ref_tour.so", dict(ref_tour_viewpoints=C.c_int32, ref_tour_select_ids=C.c_int32,
+                                                  ref_tour_pick=C.c_int32), first=ref_raycast)
 
 
 def _f64(a, shape=(-1,)):

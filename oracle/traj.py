@@ -5,31 +5,17 @@ splines, checkTrajCollision, selectBestTraj) and of the reference's own non_unif
 TEST INFRASTRUCTURE ONLY, like the rest of this package: fuel_b200/ must never import it.
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from . import _p, ref_raycast
+from . import _load, _make, _p, ref_raycast
 from . import build as _build_oracle
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "libfuel_oracle_traj.so")
-_REF_SO = os.path.join(_HERE, "_ref", "libfuel_ref_traj.so")
-_REF_SRC = "/root/reference/fuel_planner/bspline/src/non_uniform_bspline.cpp"
 
-
-def build(force=False):
+def build():
     """Compile the oracle (libfuel_oracle.so first, oracle/Makefile) and this part of it with oracle/traj.mk."""
     _build_oracle()
-    src = [os.path.join(_HERE, f) for f in ("fuel_oracle_traj.c", "fuel_oracle_traj.h", "fuel_oracle.h", "traj.mk",
-                                            "ref_traj_wrap.cpp", "libfuel_oracle.so")]
-    ref_ok = not os.path.exists(_REF_SRC) or os.path.exists(_REF_SO)
-    if (not force and os.path.exists(_SO) and ref_ok
-            and all(os.path.getmtime(_SO) >= os.path.getmtime(s) for s in src)):
-        return _SO
-    subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "traj.mk"])
-    return _SO
+    _make("traj.mk")
 
 
 class OrcTrajCheckParams(C.Structure):
@@ -40,26 +26,15 @@ TRAJ_REPORT_DTYPE = np.dtype([("duration", np.float64), ("jerk", np.float64), ("
                               ("distance", np.float64), ("safe", np.int32), ("feasible", np.int32),
                               ("n_checked", np.int32), ("reserved", np.int32)])
 
-_lib = None
-_ref = None
-
 
 def lib():
-    global _lib
-    if _lib is None:
-        build()
-        _lib = C.CDLL(_SO)
-    return _lib
+    return _load("libfuel_oracle_traj.so", {}, build=build)
 
 
 def ref_traj():
     """The REFERENCE's non_uniform_bspline.cpp + oracle/ref_traj_wrap.cpp, or None where it is not built."""
-    global _ref
-    if _ref is None and os.path.exists(_REF_SO) and ref_raycast() is not None:
-        _ref = C.CDLL(_REF_SO)
-        _ref.ref_traj_check_collision.restype = C.c_int32
-        _ref.ref_traj_select_best.restype = C.c_int32
-    return _ref
+    return _load("_ref/libfuel_ref_traj.so", dict(ref_traj_check_collision=C.c_int32, ref_traj_select_best=C.c_int32),
+                 first=ref_raycast)
 
 
 def _traj_inputs(x, n_pts, dt):

@@ -6,46 +6,23 @@ where the reference's sources are present.  The map is oracle.astar.Map.
 TEST INFRASTRUCTURE ONLY, like the rest of this package: fuel_b200/ must never import it.
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from . import _p
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SO = os.path.join(_HERE, "libfuel_oracle_view.so")
-_REF_SO = os.path.join(_HERE, "_ref", "libfuel_ref_view.so")
-_REF_SRC = "/root/reference/fuel_planner/active_perception/src/graph_node.cpp"
+from . import _load, _make, _p, ref_raycast
 
 # the layout of FuelViewCostInfo (include/fuelgpu.h)
 VIEW_DTYPE = np.dtype([("kind", np.int32), ("reason", np.int32), ("iter_num", np.int32), ("use_node_num", np.int32),
                        ("n_path", np.int32), ("reserved", np.int32), ("length", np.float64), ("cost", np.float64)])
 
 
-def build(force=False):
+def build():
     """Compile this part with oracle/view.mk."""
-    src = [os.path.join(_HERE, f) for f in ("fuel_oracle_view.c", "fuel_oracle_view.h", "fuel_oracle_astar.c",
-                                            "fuel_oracle_astar.h", "view.mk", "ref_view_wrap.cpp")]
-    ref_ok = not os.path.exists(_REF_SRC) or os.path.exists(_REF_SO)
-    if (not force and os.path.exists(_SO) and ref_ok
-            and all(os.path.getmtime(_SO) >= os.path.getmtime(s) for s in src if os.path.exists(s))):
-        return _SO
-    subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "view.mk"])
-    return _SO
-
-
-_lib = None
-_ref_view = None
+    _make("view.mk")
 
 
 def lib():
-    global _lib
-    if _lib is None:
-        build()
-        _lib = C.CDLL(_SO)
-        _lib.orc_view_cost.restype = C.c_int32
-    return _lib
+    return _load("libfuel_oracle_view.so", dict(orc_view_cost=C.c_int32), build=build)
 
 
 def view_cost_batch(m, p1, p2, y1, y2, v1, vm, yd, w_dir, resolution, lambda_heu, allocate_num, max_iter, path_max=512):
@@ -67,15 +44,9 @@ def view_cost_batch(m, p1, p2, y1, y2, v1, vm, yd, w_dir, resolution, lambda_heu
 
 
 def ref_view():
-    """The REFERENCE's graph_node.cpp + frontier_finder.cpp + oracle/ref_view_wrap.cpp, or None where it is not built."""
-    global _ref_view
-    if _ref_view is None and os.path.exists(_REF_SO):
-        from . import ref_raycast
-        ref_raycast()  # libfuel_ref.so (SDFMap, RayCaster) first
-        _ref_view = C.CDLL(_REF_SO)
-        _ref_view.ref_ffc_create.restype = C.c_void_p
-        _ref_view.ref_ffc_tour.restype = C.c_int32
-    return _ref_view
+    """The REFERENCE's graph_node.cpp + frontier_finder.cpp + oracle/ref_view_wrap.cpp over libfuel_ref.so's SDFMap and
+    RayCaster, or None where it is not built."""
+    return _load("_ref/libfuel_ref_view.so", dict(ref_ffc_create=C.c_void_p, ref_ffc_tour=C.c_int32), first=ref_raycast)
 
 
 class RefViewNode:

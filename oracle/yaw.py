@@ -14,16 +14,11 @@ TEST INFRASTRUCTURE ONLY, like the rest of this package: fuel_b200/ must never i
 """
 import ctypes as C
 import math
-import os
-import subprocess
 
 import numpy as np
 
-from . import _p, traj as _traj
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_REF_SO = os.path.join(_HERE, "_ref", "libfuel_ref_yaw.so")
-_REF_SRC = "/root/reference/fuel_planner/bspline/src/non_uniform_bspline.cpp"
+from . import _load, _make, _p, ref_raycast, traj as _traj
+from . import build as _build_oracle
 
 SEG_NUM = 12                # planYawExplore's seg_num
 PTS = SEG_NUM + 3           # yaw control points
@@ -33,18 +28,10 @@ OK, BAD_INPUT, RELAX_OVERFLOW, NO_LOOKAHEAD, ZERO_PT_DIST, NOT_SPD = range(6)  #
 YAW_MASK = 1 | 8 | 16 | 64  # SMOOTHNESS | START | END | WAYPOINTS
 
 
-def build(force=False):
+def build():
     """Compile the reference's side with oracle/yaw.mk (needs oracle/_ref/libfuel_ref.so from the Makefile first)."""
-    from . import build as _build_oracle
     _build_oracle()
-    if not os.path.exists(_REF_SRC):
-        return None
-    src = [os.path.join(_HERE, f) for f in ("yaw.mk", "ref_yaw_wrap.cpp", "ref_yaw_cost_wrap.cpp")]
-    if (not force and os.path.exists(_REF_SO)
-            and all(os.path.getmtime(_REF_SO) >= os.path.getmtime(s) for s in src)):
-        return _REF_SO
-    subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "yaw.mk"])
-    return _REF_SO
+    _make("yaw.mk")
 
 
 def wrap_start(y):
@@ -254,21 +241,10 @@ def objective(rows, q, ld_smooth=20.0, ld_start=100.0, ld_end=0.5, ld_waypt=0.3)
 
 
 # ---- the reference's own code ------------------------------------------------------------------------------------------
-_ref = None
-
-
 def ref_yaw():
     """oracle/_ref/libfuel_ref_yaw.so (the reference's non_uniform_bspline.cpp + ref_yaw_wrap.cpp, and
     ref_yaw_cost_wrap.cpp over _ref/libfuel_ref.so's BsplineOptimizer), or None where it is not built."""
-    global _ref
-    if _ref is None and os.path.exists(_REF_SO):
-        from . import ref_raycast
-        if ref_raycast() is None:
-            return None
-        _ref = C.CDLL(_REF_SO)
-        _ref.ref_yaw_explore.restype = C.c_int32
-        _ref.ref_yaw_cost.restype = C.c_int32
-    return _ref
+    return _load("_ref/libfuel_ref_yaw.so", dict(ref_yaw_explore=C.c_int32, ref_yaw_cost=C.c_int32), first=ref_raycast)
 
 
 def ref_plan(ctrl, dt, start_yaw, end_yaw, relax_time=1.0, lookfwd=True):

@@ -1,10 +1,11 @@
 """What the reference's own code computes, for the tests that pin the oracle to it.
 
-Where oracle/_ref/libfuel_ref.so is built (oracle/Makefile, from the reference's sources), the tests run the reference
-and compare the oracle with it directly; every reference result is also checked against its SHA-256 digest in
-tests/golden/refpin.json, so the stored digests cannot drift from the code they stand for.  Everywhere else the digests
-stand in for the reference: the oracle's result must hash to the digest of the reference's.  Values are hashed as
-float64 arrays (shape included, -0.0 as 0.0, every NaN alike), so a digest match is np.array_equal with NaN == NaN.
+Where the reference's library is built (oracle/_ref, from the reference's sources), the tests run the reference and
+compare the oracle with it directly; every reference result is also checked against its SHA-256 digest in the module's
+golden file under tests/golden/ (refpin.json unless the module names another), so the stored digests cannot drift from
+the code they stand for.  Everywhere else the digests stand in for the reference: the oracle's result must hash to the
+digest of the reference's.  Values are hashed as float64 arrays (shape included, -0.0 as 0.0, every NaN alike), so a
+digest match is np.array_equal with NaN == NaN.
 
   FUEL_REFPIN_RECORD=1 python -m pytest tests/test_oracle_refpin.py tests/test_host_frontier_bookkeeping.py
 
@@ -16,10 +17,11 @@ import math
 import os
 
 import numpy as np
+import pytest
 
 import oracle as O
 
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "refpin.json")
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 RECORD = os.environ.get("FUEL_REFPIN_RECORD") == "1"
 
 
@@ -73,13 +75,15 @@ def first_difference(a, b, path=""):
 
 
 class RefGold:
-    """One per test: eq(got, lambda: <the reference's value>) in the order the test makes its comparisons."""
+    """One per test: eq(got, lambda: <the reference's value>) in the order the test makes its comparisons.  The digests
+    are in tests/golden/<gold>; the reference runs where live() is not None."""
 
-    def __init__(self, test_id):
-        self.live = O.ref_raycast() is not None
+    def __init__(self, test_id, gold="refpin.json", live=O.ref_raycast):
+        self.live = live() is not None
         self.test_id = test_id
+        self.gold = os.path.join(GOLDEN, gold)
         self.count = 0
-        self.stored = json.load(open(GOLD)) if os.path.exists(GOLD) else {}
+        self.stored = json.load(open(self.gold)) if os.path.exists(self.gold) else {}
         self.recorded = {}
 
     def eq(self, got, reference):
@@ -92,19 +96,33 @@ class RefGold:
             d = digest(want)
             self.recorded[key] = d
             if not RECORD:
-                assert self.stored.get(key) == d, "%s: %s is out of date (FUEL_REFPIN_RECORD=1 rewrites it)" % (key, GOLD)
+                assert self.stored.get(key) == d, "%s: %s is out of date (FUEL_REFPIN_RECORD=1 rewrites it)" % (
+                    key, self.gold)
         else:
-            assert key in self.stored, "%s: no stored reference result in %s" % (key, GOLD)
+            assert key in self.stored, "%s: no stored reference result in %s" % (key, self.gold)
             assert digest(got) == self.stored[key], "%s: the oracle no longer computes what the reference computed" % key
 
     def finish(self):
         if self.live and RECORD:
-            d = json.load(open(GOLD)) if os.path.exists(GOLD) else {}
+            d = json.load(open(self.gold)) if os.path.exists(self.gold) else {}
             d = {k: v for k, v in d.items() if not k.startswith(self.test_id + "#")}
             d.update(self.recorded)
-            with open(GOLD, "w") as f:
+            with open(self.gold, "w") as f:
                 json.dump(dict(sorted(d.items())), f, indent=0)
                 f.write("\n")
+
+
+def refgold_fixture(gold="refpin.json", live=O.ref_raycast):
+    """The per-test fixture G of a module whose digests are in tests/golden/<gold>, live where live() is not None:
+    G = refgold_fixture(...) at the module's top level."""
+
+    @pytest.fixture
+    def G(request):
+        g = RefGold("%s::%s" % (request.module.__name__.split(".")[-1], request.node.name), gold, live)
+        yield g
+        g.finish()
+
+    return G
 
 
 class MapGeometry:

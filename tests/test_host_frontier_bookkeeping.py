@@ -5,12 +5,11 @@ here (no GPU needed), so what is compared is exactly the host logic: which store
 changes (haveOverlap + isFrontierChanged), removed_ids_, the dormant list, id assignment, viewpoint filtering / order.
 Where oracle/_ref is not built, the digests of the reference's results stand in for it (tests/refgold.py)."""
 import numpy as np
-import pytest
 
 import oracle as O
 from fuel_b200 import workloads as W
 from fuel_b200.frontier_finder import Frontier, FrontierFinder
-from tests.refgold import RefGold, ref_map
+from tests.refgold import ref_map, refgold_fixture
 
 O.build()
 
@@ -90,11 +89,7 @@ def visit_list(lst):
     return out
 
 
-@pytest.fixture
-def G(request):
-    g = RefGold("%s::%s" % (request.module.__name__.split(".")[-1], request.node.name))
-    yield g
-    g.finish()
+G = refgold_fixture()
 
 
 def test_exploration_episode_matches_reference(G):

@@ -9,20 +9,16 @@ in for it.
   FUEL_REFPIN_RECORD=1 python -m pytest tests/test_oracle_astar.py
 
 rewrites the digests from a run against the built reference."""
-import json
-import os
-
 import numpy as np
 import pytest
 
 import oracle as O
 import oracle.astar as OA
 from fuel_b200 import workloads as W
-from tests.refgold import RECORD, digest, first_difference
+from tests.refgold import refgold_fixture
 
 OA.build()
 
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "refpin_astar.json")
 PATH_MAX, W_MAX = 512, 32
 
 
@@ -30,47 +26,7 @@ def logit(p):
     return np.log(p / (1 - p))
 
 
-class AstarRefGold:
-    """the reference's result where libfuel_ref_astar.so is built (and the stored digest kept current), the stored
-    digest elsewhere"""
-
-    def __init__(self, test_id):
-        self.live = OA.ref_astar() is not None
-        self.test_id = test_id
-        self.count = 0
-        self.stored = json.load(open(GOLD)) if os.path.exists(GOLD) else {}
-        self.recorded = {}
-
-    def eq(self, got, reference):
-        key = "%s#%d" % (self.test_id, self.count)
-        self.count += 1
-        if self.live:
-            want = reference()
-            diff = first_difference(got, want)
-            assert diff is None, "%s: oracle vs reference%s" % (key, diff)
-            self.recorded[key] = digest(want)
-            if not RECORD:
-                assert self.stored.get(key) == self.recorded[key], "%s: %s is out of date (FUEL_REFPIN_RECORD=1)" % (
-                    key, GOLD)
-        else:
-            assert key in self.stored, "%s: no stored reference result in %s" % (key, GOLD)
-            assert digest(got) == self.stored[key], "%s: the oracle no longer computes what the reference computed" % key
-
-    def finish(self):
-        if self.live and RECORD:
-            d = json.load(open(GOLD)) if os.path.exists(GOLD) else {}
-            d = {k: v for k, v in d.items() if not k.startswith(self.test_id + "#")}
-            d.update(self.recorded)
-            with open(GOLD, "w") as f:
-                json.dump(dict(sorted(d.items())), f, indent=0)
-                f.write("\n")
-
-
-@pytest.fixture
-def G(request):
-    g = AstarRefGold("%s::%s" % (request.module.__name__.split(".")[-1], request.node.name))
-    yield g
-    g.finish()
+G = refgold_fixture("refpin_astar.json", OA.ref_astar)
 
 
 def flat(res):

@@ -8,9 +8,6 @@ the reference library is not built, the digests in tests/golden/refpin_kino.json
   FUEL_REFPIN_RECORD=1 python -m pytest tests/test_oracle_kino_refpin.py
 
 rewrites the digests from a run against the built reference."""
-import json
-import os
-
 import numpy as np
 import pytest
 
@@ -19,11 +16,10 @@ import oracle.kino as OK
 from fuel_b200 import workloads as W
 from fuel_b200.kino_astar import make_params
 from tests.kino_cases import hand_cases, mid_queries
-from tests.refgold import RECORD, digest, first_difference
+from tests.refgold import refgold_fixture
 
 OK.build()
 
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "refpin_kino.json")
 NODE_MAX = 128
 # kinodynamic_astar.cpp's reasons are not outputs of the reference: the wrapper infers them, so they are left out
 FIELDS = ("status", "retried", "traj_status", "iter_num", "use_node_num", "n_nodes", "shot", "seg_num", "n_pts",
@@ -34,44 +30,7 @@ def logit(p):
     return np.log(p / (1 - p))
 
 
-class KinoRefGold:
-    def __init__(self, test_id):
-        self.live = OK.ref_kino() is not None
-        self.test_id = test_id
-        self.count = 0
-        self.stored = json.load(open(GOLD)) if os.path.exists(GOLD) else {}
-        self.recorded = {}
-
-    def eq(self, got, reference):
-        key = "%s#%d" % (self.test_id, self.count)
-        self.count += 1
-        if self.live:
-            want = reference()
-            diff = first_difference(got, want)
-            assert diff is None, "%s: oracle vs reference%s" % (key, diff)
-            self.recorded[key] = digest(want)
-            if not RECORD:
-                assert self.stored.get(key) == self.recorded[key], "%s: %s is out of date (FUEL_REFPIN_RECORD=1)" % (
-                    key, GOLD)
-        else:
-            assert key in self.stored, "%s: no stored reference result in %s" % (key, GOLD)
-            assert digest(got) == self.stored[key], "%s: the oracle no longer computes what the reference computed" % key
-
-    def finish(self):
-        if self.live and RECORD:
-            d = json.load(open(GOLD)) if os.path.exists(GOLD) else {}
-            d = {k: v for k, v in d.items() if not k.startswith(self.test_id + "#")}
-            d.update(self.recorded)
-            with open(GOLD, "w") as f:
-                json.dump(dict(sorted(d.items())), f, indent=0)
-                f.write("\n")
-
-
-@pytest.fixture
-def G(request):
-    g = KinoRefGold("%s::%s" % (request.module.__name__.split(".")[-1], request.node.name))
-    yield g
-    g.finish()
+G = refgold_fixture("refpin_kino.json", OK.ref_kino)
 
 
 def flat(r):

@@ -12,9 +12,6 @@ tests/golden/refpin_tour.json stand in for it.
 rewrites the digests from a run against the built reference.  The other tests here check the oracle's own parts: the
 lazy search equals the same search over its own edge costs, std::priority_queue's tie order, the unreachable and
 zero-length-segment branches."""
-import json
-import os
-
 import numpy as np
 import pytest
 
@@ -23,12 +20,10 @@ import oracle.tour as OT
 from fuel_b200 import exploration_manager as EM
 from fuel_b200 import workloads as W
 from fuel_b200.frontier_finder import FrontierFinder
-from tests.refgold import RECORD, digest, first_difference
+from tests.refgold import refgold_fixture
 from tests.test_oracle_astar import Scene
 
 OT.build()
-
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "refpin_tour.json")
 
 VM, YD, W_DIR = 2.0, 60 * 3.1415926 / 180.0, 1.5  # exploration/vm (max_vel 2.0), yd, w_dir: algorithm.xml:95-99
 PRM = (VM, YD, W_DIR, 0.4, 10000.0, 100000, 400)
@@ -160,47 +155,7 @@ def test_select_refined_ids():
 
 
 # ---- pinned on the compiled reference -------------------------------------------------------------------------------
-class TourRefGold:
-    """the reference's result where libfuel_ref_tour.so is built (and the stored digest kept current), the stored
-    digest elsewhere"""
-
-    def __init__(self, test_id):
-        self.live = OT.ref_tour() is not None
-        self.test_id = test_id
-        self.count = 0
-        self.stored = json.load(open(GOLD)) if os.path.exists(GOLD) else {}
-        self.recorded = {}
-
-    def eq(self, got, reference):
-        key = "%s#%d" % (self.test_id, self.count)
-        self.count += 1
-        if self.live:
-            want = reference()
-            diff = first_difference(got, want)
-            assert diff is None, "%s: oracle vs reference%s" % (key, diff)
-            self.recorded[key] = digest(want)
-            if not RECORD:
-                assert self.stored.get(key) == self.recorded[key], "%s: %s is out of date (FUEL_REFPIN_RECORD=1)" % (
-                    key, GOLD)
-        else:
-            assert key in self.stored, "%s: no stored reference result in %s" % (key, GOLD)
-            assert digest(got) == self.stored[key], "%s: the oracle no longer computes what the reference computed" % key
-
-    def finish(self):
-        if self.live and RECORD:
-            d = json.load(open(GOLD)) if os.path.exists(GOLD) else {}
-            d = {k: v for k, v in d.items() if not k.startswith(self.test_id + "#")}
-            d.update(self.recorded)
-            with open(GOLD, "w") as f:
-                json.dump(dict(sorted(d.items())), f, indent=0)
-                f.write("\n")
-
-
-@pytest.fixture
-def G(request):
-    g = TourRefGold("%s::%s" % (request.module.__name__.split(".")[-1], request.node.name))
-    yield g
-    g.finish()
+G = refgold_fixture("refpin_tour.json", OT.ref_tour)
 
 
 @pytest.fixture(scope="module", params=["office", "office3"])

@@ -10,63 +10,17 @@ tests/golden/refpin_poly.json stand in for it.
   FUEL_REFPIN_RECORD=1 python -m pytest tests/test_oracle_poly.py
 
 rewrites the digests from a run against the built reference."""
-import json
-import os
-
 import numpy as np
 import pytest
 
 import oracle.poly as O
 from fuel_b200 import workloads as W
 from tests.poly_cases import GRID_S, exact_minjerk, grid_cases, poly_eval, random_tour
-from tests.refgold import RECORD, digest, first_difference
+from tests.refgold import refgold_fixture
 
 O.build()
 
-GOLD_POLY = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "refpin_poly.json")
-
-
-class PolyRefGold:
-    """the reference's result where its polynomial_traj.cpp is built (and the stored digest kept current), the stored
-    digest elsewhere"""
-
-    def __init__(self, test_id):
-        self.live = O.ref_poly() is not None
-        self.test_id = test_id
-        self.count = 0
-        self.stored = json.load(open(GOLD_POLY)) if os.path.exists(GOLD_POLY) else {}
-        self.recorded = {}
-
-    def eq(self, got, reference):
-        key = "%s#%d" % (self.test_id, self.count)
-        self.count += 1
-        if self.live:
-            want = reference()
-            diff = first_difference(got, want)
-            assert diff is None, "%s: oracle vs reference%s" % (key, diff)
-            self.recorded[key] = digest(want)
-            if not RECORD:
-                assert self.stored.get(key) == self.recorded[key], "%s: %s is out of date (FUEL_REFPIN_RECORD=1)" % (
-                    key, GOLD_POLY)
-        else:
-            assert key in self.stored, "%s: no stored reference result in %s" % (key, GOLD_POLY)
-            assert digest(got) == self.stored[key], "%s: the oracle no longer computes what the reference computed" % key
-
-    def finish(self):
-        if self.live and RECORD:
-            d = json.load(open(GOLD_POLY)) if os.path.exists(GOLD_POLY) else {}
-            d = {k: v for k, v in d.items() if not k.startswith(self.test_id + "#")}
-            d.update(self.recorded)
-            with open(GOLD_POLY, "w") as f:
-                json.dump(dict(sorted(d.items())), f, indent=0)
-                f.write("\n")
-
-
-@pytest.fixture
-def G(request):
-    g = PolyRefGold("%s::%s" % (request.module.__name__.split(".")[-1], request.node.name))
-    yield g
-    g.finish()
+G = refgold_fixture("refpin_poly.json", O.ref_poly)
 
 
 def _tour(S, seed):

@@ -10,16 +10,12 @@ import numpy as np
 import pytest
 
 import oracle as O
-from tests.refgold import RefGold, ref_map
+from tests.refgold import ref_map, refgold_fixture
 
 O.build()  # also builds oracle/_ref/libfuel_ref.so where the reference's sources are present (it is git-ignored)
 
 
-@pytest.fixture
-def G(request):
-    g = RefGold("%s::%s" % (request.module.__name__.split(".")[-1], request.node.name))
-    yield g
-    g.finish()
+G = refgold_fixture()
 
 
 def test_intbound_matches_reference(G):

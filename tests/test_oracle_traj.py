@@ -9,9 +9,6 @@ derivative, and a brute-force sequential collision scan.
   FUEL_REFPIN_RECORD=1 python -m pytest tests/test_oracle_traj.py
 
 rewrites the digests from a run against the built reference."""
-import json
-import os
-
 import numpy as np
 import pytest
 from scipy.interpolate import BSpline
@@ -19,47 +16,9 @@ from scipy.interpolate import BSpline
 import oracle.traj as O
 from oracle import make_grid as O_grid
 from fuel_b200 import workloads as W
-from tests.refgold import RECORD, RefGold, digest, first_difference, ref_map
+from tests.refgold import ref_map, refgold_fixture
 
 O.build()  # also builds oracle/_ref/libfuel_ref_traj.so where the reference's sources are present (git-ignored)
-
-GOLD_TRAJ = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "refpin_traj.json")
-
-
-class TrajRefGold(RefGold):
-    """RefGold with the digests of this file's comparisons in their own golden file, live where the reference's
-    non_uniform_bspline.cpp is built"""
-
-    def __init__(self, test_id):
-        self.live = O.ref_traj() is not None
-        self.test_id = test_id
-        self.count = 0
-        self.stored = json.load(open(GOLD_TRAJ)) if os.path.exists(GOLD_TRAJ) else {}
-        self.recorded = {}
-
-    def eq(self, got, reference):
-        key = "%s#%d" % (self.test_id, self.count)
-        self.count += 1
-        if self.live:
-            want = reference()
-            diff = first_difference(got, want)
-            assert diff is None, "%s: oracle vs reference%s" % (key, diff)
-            self.recorded[key] = digest(want)
-            if not RECORD:
-                assert self.stored.get(key) == self.recorded[key], "%s: %s is out of date (FUEL_REFPIN_RECORD=1)" % (
-                    key, GOLD_TRAJ)
-        else:
-            assert key in self.stored, "%s: no stored reference result in %s" % (key, GOLD_TRAJ)
-            assert digest(got) == self.stored[key], "%s: the oracle no longer computes what the reference computed" % key
-
-    def finish(self):
-        if self.live and RECORD:
-            d = json.load(open(GOLD_TRAJ)) if os.path.exists(GOLD_TRAJ) else {}
-            d = {k: v for k, v in d.items() if not k.startswith(self.test_id + "#")}
-            d.update(self.recorded)
-            with open(GOLD_TRAJ, "w") as f:
-                json.dump(dict(sorted(d.items())), f, indent=0)
-                f.write("\n")
 
 
 BASE = dict(resolution=0.1, map_size_x=8.0, map_size_y=6.0, map_size_z=3.0, ground_height=-0.5, obstacles_inflation=0.199,
@@ -67,11 +26,7 @@ BASE = dict(resolution=0.1, map_size_x=8.0, map_size_y=6.0, map_size_z=3.0, grou
             p_miss=0.35, p_min=0.12, p_max=0.90, p_occ=0.80, max_ray_length=4.5, virtual_ceil_height=-10.0)
 
 
-@pytest.fixture
-def G(request):
-    g = TrajRefGold("%s::%s" % (request.module.__name__.split(".")[-1], request.node.name))
-    yield g
-    g.finish()
+G = refgold_fixture("refpin_traj.json", O.ref_traj)
 
 
 def random_trajs(rng, B, n, lo=(-3.5, -2.5, 0.0), hi=(3.5, 2.5, 2.0), step=0.25, dt_range=(0.05, 0.6)):

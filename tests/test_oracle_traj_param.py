@@ -10,67 +10,22 @@ in for it (tests/refgold.py's scheme).
   FUEL_REFPIN_RECORD=1 python -m pytest tests/test_oracle_traj_param.py
 
 rewrites the digests from a run against the built reference."""
-import json
-import os
-
 import numpy as np
 import pytest
 
 import oracle as OR
 import oracle.param as O
 from tests.param_cases import GRID_DT, GRID_K, exact_lstsq, noisy_samples, spline_samples
-from tests.refgold import RECORD, RefGold, digest, first_difference
+from tests.refgold import refgold_fixture
 
 O.build()
-
-GOLD_PARAM = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "refpin_param.json")
 
 # the (K, dt) grid of the rank and reference checks
 RANK_K = (2, 3, 4, 8, 18, 30, 31, 62)
 RANK_DT = (0.02, 0.05, 0.1, 0.175, 0.35, 1.0, 5.0)
 
 
-class ParamRefGold(RefGold):
-    """RefGold with this file's digests in their own golden file, live where the reference's non_uniform_bspline.cpp
-    is built"""
-
-    def __init__(self, test_id):
-        self.live = O.ref_param() is not None
-        self.test_id = test_id
-        self.count = 0
-        self.stored = json.load(open(GOLD_PARAM)) if os.path.exists(GOLD_PARAM) else {}
-        self.recorded = {}
-
-    def eq(self, got, reference):
-        key = "%s#%d" % (self.test_id, self.count)
-        self.count += 1
-        if self.live:
-            want = reference()
-            diff = first_difference(got, want)
-            assert diff is None, "%s: oracle vs reference%s" % (key, diff)
-            self.recorded[key] = digest(want)
-            if not RECORD:
-                assert self.stored.get(key) == self.recorded[key], "%s: %s is out of date (FUEL_REFPIN_RECORD=1)" % (
-                    key, GOLD_PARAM)
-        else:
-            assert key in self.stored, "%s: no stored reference result in %s" % (key, GOLD_PARAM)
-            assert digest(got) == self.stored[key], "%s: the oracle no longer computes what the reference computed" % key
-
-    def finish(self):
-        if self.live and RECORD:
-            d = json.load(open(GOLD_PARAM)) if os.path.exists(GOLD_PARAM) else {}
-            d = {k: v for k, v in d.items() if not k.startswith(self.test_id + "#")}
-            d.update(self.recorded)
-            with open(GOLD_PARAM, "w") as f:
-                json.dump(dict(sorted(d.items())), f, indent=0)
-                f.write("\n")
-
-
-@pytest.fixture
-def G(request):
-    g = ParamRefGold("%s::%s" % (request.module.__name__.split(".")[-1], request.node.name))
-    yield g
-    g.finish()
+G = refgold_fixture("refpin_param.json", O.ref_param)
 
 
 # ---- against the reference's own code ------------------------------------------------------------------------------

@@ -10,9 +10,6 @@ tests/golden/refpin_view_cost.json stand in for it.
   FUEL_REFPIN_RECORD=1 python -m pytest tests/test_oracle_view_cost.py
 
 rewrites the digests from a run against the built reference."""
-import json
-import os
-
 import numpy as np
 import pytest
 
@@ -20,57 +17,16 @@ import oracle.astar as OA
 import oracle.view as OV
 from fuel_b200 import frontier_finder as FF
 from fuel_b200 import workloads as W
-from tests.refgold import RECORD, digest, first_difference
+from tests.refgold import refgold_fixture
 from tests.test_oracle_astar import Scene
 
 OV.build()
 
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "refpin_view_cost.json")
 PATH_MAX = 512
 VM, YD, W_DIR = 2.0, 60 * 3.1415926 / 180.0, 1.5  # exploration/vm (max_vel 2.0), yd, w_dir: algorithm.xml:95-99
 
 
-class ViewRefGold:
-    """the reference's result where libfuel_ref_view.so is built (and the stored digest kept current), the stored
-    digest elsewhere"""
-
-    def __init__(self, test_id):
-        self.live = OV.ref_view() is not None
-        self.test_id = test_id
-        self.count = 0
-        self.stored = json.load(open(GOLD)) if os.path.exists(GOLD) else {}
-        self.recorded = {}
-
-    def eq(self, got, reference):
-        key = "%s#%d" % (self.test_id, self.count)
-        self.count += 1
-        if self.live:
-            want = reference()
-            diff = first_difference(got, want)
-            assert diff is None, "%s: oracle vs reference%s" % (key, diff)
-            self.recorded[key] = digest(want)
-            if not RECORD:
-                assert self.stored.get(key) == self.recorded[key], "%s: %s is out of date (FUEL_REFPIN_RECORD=1)" % (
-                    key, GOLD)
-        else:
-            assert key in self.stored, "%s: no stored reference result in %s" % (key, GOLD)
-            assert digest(got) == self.stored[key], "%s: the oracle no longer computes what the reference computed" % key
-
-    def finish(self):
-        if self.live and RECORD:
-            d = json.load(open(GOLD)) if os.path.exists(GOLD) else {}
-            d = {k: v for k, v in d.items() if not k.startswith(self.test_id + "#")}
-            d.update(self.recorded)
-            with open(GOLD, "w") as f:
-                json.dump(dict(sorted(d.items())), f, indent=0)
-                f.write("\n")
-
-
-@pytest.fixture
-def G(request):
-    g = ViewRefGold("%s::%s" % (request.module.__name__.split(".")[-1], request.node.name))
-    yield g
-    g.finish()
+G = refgold_fixture("refpin_view_cost.json", OV.ref_view)
 
 
 def flat(res):

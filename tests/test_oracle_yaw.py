@@ -9,67 +9,24 @@ is not built, the digests in tests/golden/refpin_yaw.json stand in for it.
   FUEL_REFPIN_RECORD=1 python -m pytest tests/test_oracle_yaw.py
 
 rewrites the digests from a run against the built reference."""
-import json
 import math
-import os
 
 import numpy as np
 import pytest
 
 import oracle.yaw as OY
 from fuel_b200 import workloads as W
-from tests.refgold import RECORD, digest, first_difference, ref_map
+from tests.refgold import ref_map, refgold_fixture
 from tests.yaw_cases import DT_YAW_GRID, LD, arc_batch, exact_minimizer, solve_bar
 
 OY.build()
 
-GOLD_YAW = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "refpin_yaw.json")
 MAP = dict(resolution=0.1, map_size_x=8.0, map_size_y=6.0, map_size_z=3.0, ground_height=-0.5, obstacles_inflation=0.199,
            local_bound_inflate=0.5, local_map_margin=50, default_dist=0.0, optimistic=0, signed_dist=0, p_hit=0.65,
            p_miss=0.35, p_min=0.12, p_max=0.90, p_occ=0.80, max_ray_length=4.5, virtual_ceil_height=-10.0)
 
 
-class YawRefGold:
-    """the reference's result where libfuel_ref_yaw.so is built (and the stored digest kept current), the stored digest
-    elsewhere"""
-
-    def __init__(self, test_id):
-        self.live = OY.ref_yaw() is not None
-        self.test_id = test_id
-        self.count = 0
-        self.stored = json.load(open(GOLD_YAW)) if os.path.exists(GOLD_YAW) else {}
-        self.recorded = {}
-
-    def eq(self, got, reference):
-        key = "%s#%d" % (self.test_id, self.count)
-        self.count += 1
-        if self.live:
-            want = reference()
-            diff = first_difference(got, want)
-            assert diff is None, "%s: oracle vs reference%s" % (key, diff)
-            self.recorded[key] = digest(want)
-            if not RECORD:
-                assert self.stored.get(key) == self.recorded[key], "%s: %s is out of date (FUEL_REFPIN_RECORD=1)" % (
-                    key, GOLD_YAW)
-        else:
-            assert key in self.stored, "%s: no stored reference result in %s" % (key, GOLD_YAW)
-            assert digest(got) == self.stored[key], "%s: the oracle no longer computes what the reference computed" % key
-
-    def finish(self):
-        if self.live and RECORD:
-            d = json.load(open(GOLD_YAW)) if os.path.exists(GOLD_YAW) else {}
-            d = {k: v for k, v in d.items() if not k.startswith(self.test_id + "#")}
-            d.update(self.recorded)
-            with open(GOLD_YAW, "w") as f:
-                json.dump(dict(sorted(d.items())), f, indent=0)
-                f.write("\n")
-
-
-@pytest.fixture
-def G(request):
-    g = YawRefGold("%s::%s" % (request.module.__name__.split(".")[-1], request.node.name))
-    yield g
-    g.finish()
+G = refgold_fixture("refpin_yaw.json", OY.ref_yaw)
 
 
 def pinned(r):
