@@ -89,6 +89,11 @@ class FuelYawInfo(C.Structure):
     _fields_ = [("dt_yaw", C.c_double), ("pt_dist", C.c_double), ("n_waypt", C.c_int32), ("status", C.c_int32)]
 
 
+class FuelPlanYawInfo(C.Structure):
+    _fields_ = [("dt_yaw", C.c_double), ("pt_dist", C.c_double), ("seg_num", C.c_int32), ("n_waypt", C.c_int32),
+                ("status", C.c_int32), ("reserved", C.c_int32)]
+
+
 class FuelAstarParams(C.Structure):
     _fields_ = [("resolution", C.c_double), ("lambda_heu", C.c_double), ("allocate_num", C.c_int32),
                 ("max_iter", C.c_int32)]
@@ -203,6 +208,9 @@ SIGNATURES = {
                                             C.POINTER(FuelYawParams), _vp, _vp, _vp]),
     "fuelgpu_yaw_explore_batch_dev": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, C.POINTER(FuelOptParams),
                                                 C.POINTER(FuelYawParams), _vp, _vp, _vp]),
+    "fuelgpu_plan_yaw_batch": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, C.POINTER(FuelOptParams), _vp, _vp, _vp]),
+    "fuelgpu_plan_yaw_batch_dev": (C.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, C.POINTER(FuelOptParams), _vp, _vp,
+                                             _vp]),
     "fuelgpu_astar_batch": (C.c_int, [_vp, _i32, _vp, _vp, C.POINTER(FuelAstarParams), _vp, _i32, _vp, _i32, _vp, _vp]),
     "fuelgpu_astar_batch_dev": (C.c_int, [_vp, _i32, _vp, _vp, C.POINTER(FuelAstarParams), _vp, _i32, _vp, _i32, _vp,
                                           _vp]),

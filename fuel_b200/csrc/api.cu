@@ -1251,6 +1251,57 @@ int fuelgpu_yaw_explore_batch(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar
   return st.download();
 }
 
+static int check_plan_yaw_args(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar, const void* x, const void* dt,
+                               const void* start_yaw, const FuelOptParams* p, const void* yaw, const void* info) {
+  int rc = check_traj_args(m, B, n_pts, nvar, x != nullptr, dt != nullptr);
+  if (rc) return rc;
+  if (!p) return fuel_fail(m, FUELGPU_EINVAL, "null params");
+  if (!finite_pos(p->ld_smooth) || !finite_pos(p->ld_start))
+    return fuel_fail(m, FUELGPU_EINVAL, "ld_smooth and ld_start must be finite and positive");
+  if (B > 0 && (!start_yaw || !yaw || !info)) return fuel_fail(m, FUELGPU_EINVAL, "null argument");
+  return 0;
+}
+
+int fuelgpu_plan_yaw_batch_dev(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar, const void* x_dev,
+                               const void* dt_dev, const void* start_yaw_dev, const FuelOptParams* p, void* yaw_dev,
+                               void* info_dev, void* waypt_dev) {
+  int rc = check_plan_yaw_args(m, B, n_pts, nvar, x_dev, dt_dev, start_yaw_dev, p, yaw_dev, info_dev);
+  if (rc) return rc;
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  return plan_yaw_impl(m, B, n_pts, nvar, (const double*)x_dev, (const double*)dt_dev, (const double*)start_yaw_dev, p,
+                       (double*)yaw_dev, (FuelPlanYawInfo*)info_dev, (double*)waypt_dev);
+}
+
+int fuelgpu_plan_yaw_batch(FuelMap* m, int32_t B, int32_t n_pts, int32_t nvar, const double* x, const double* dt,
+                           const double* start_yaw, const FuelOptParams* p, double* yaw, FuelPlanYawInfo* info,
+                           double* waypt) {
+  int rc = check_plan_yaw_args(m, B, n_pts, nvar, x, dt, start_yaw, p, yaw, info);
+  if (rc) return rc;
+  for (int32_t b = 0; b < B; ++b) {
+    const double d = dt ? dt[b] : x[(size_t)b * nvar + 3 * n_pts];
+    if (!finite_pos(d)) return fuel_fail(m, FUELGPU_EINVAL, "dt of trajectory %s%lld must be finite and positive", "",
+                                         (long long)b);
+    const double* s = start_yaw + 3 * (size_t)b;
+    // bounds calcNextYaw's wrapping loops (planner_manager.cpp:869-870), which never end on a non-finite yaw
+    if (!(fabs(s[0]) <= FUELGPU_YAW_MAX_START) || !isfinite(s[1]) || !isfinite(s[2]))
+      return fuel_fail(m, FUELGPU_EINVAL, "trajectory %s%lld: start yaw must be finite with |yaw| <= 1000", "",
+                       (long long)b);
+  }
+  if (B == 0) return 0;
+  FUEL_CUDA(m, cudaSetDevice(m->dev));
+  const size_t nb = (size_t)B;
+  double *d_x, *d_dt, *d_sy, *d_yaw, *d_wp;
+  FuelPlanYawInfo* d_info;
+  HostStaging st(m);
+  st.in(&d_x, x, nb * nvar).in(&d_dt, dt, nb).in(&d_sy, start_yaw, nb * 3);
+  st.out(&d_yaw, yaw, nb * FUELGPU_PLANYAW_MAX_PTS).out(&d_info, info, nb).out(&d_wp, waypt, nb * FUELGPU_PLANYAW_MAX_SEG);
+  rc = st.upload();
+  if (rc) return rc;
+  rc = plan_yaw_impl(m, B, n_pts, nvar, d_x, d_dt, d_sy, p, d_yaw, d_info, d_wp);
+  if (rc) return rc;
+  return st.download();
+}
+
 static int check_astar_params(FuelMap* m, const FuelAstarParams* p) {
   if (!p) return fuel_fail(m, FUELGPU_EINVAL, "null params");
   // above 1e-3 the reference's neighbour loop (astar2.cpp:90-94) makes exactly the 26 steps

@@ -234,6 +234,9 @@ int traj_param_impl(FuelMap* m, int B, int n_pts, int nvar, const double* pts_de
 int yaw_explore_impl(FuelMap* m, int B, int n_pts, int nvar, const double* x_dev, const double* dt_dev,
                      const double* syaw_dev, const double* eyaw_dev, const FuelOptParams* p, const FuelYawParams* yp,
                      double* yaw_dev, FuelYawInfo* info_dev, double* wpt_dev);
+int plan_yaw_impl(FuelMap* m, int B, int n_pts, int nvar, const double* x_dev, const double* dt_dev,
+                  const double* syaw_dev, const FuelOptParams* p, double* yaw_dev, FuelPlanYawInfo* info_dev,
+                  double* wpt_dev);
 // poly_traj.cu: waypointsTraj + getLength + planExploreTraj's sampling (planner_manager.cpp:270-297)
 int poly_waypoints_impl(FuelMap* m, int B, int w_max, const int32_t* n_wp_dev, const double* wp_dev,
                         const double* sv_dev, const double* sa_dev, const double* ev_dev, const double* ea_dev,

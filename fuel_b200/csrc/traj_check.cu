@@ -448,16 +448,47 @@ __device__ __forceinline__ double next_yaw(double last_yaw, double yaw) {
   return last_yaw + diff + 2 * YAW_PI;
 }
 
-// w * (a . q - t)^2 over control points o .. o + L - 1, added to H and r (the objective's Hessian and gradient at 0,
-// both halved)
+// w * (a . q - t)^2 over control points o .. o + L - 1, added to H (band Hb[i][d] = H(i, i - d)) and r (the objective's
+// Hessian and gradient at 0, both halved)
 template <int L>
-__device__ __forceinline__ void yaw_term(YawSmem& y, int o, const double (&a)[L], double w, double t) {
+__device__ __forceinline__ void yaw_term(double (*Hb)[4], double* r, int o, const double (&a)[L], double w, double t) {
 #pragma unroll
   for (int u = 0; u < L; ++u) {
 #pragma unroll
-    for (int v = 0; v <= u; ++v) y.Hb[o + u][u - v] += (w * a[u]) * a[v];
-    y.r[o + u] += (w * a[u]) * t;
+    for (int v = 0; v <= u; ++v) Hb[o + u][u - v] += (w * a[u]) * a[v];
+    r[o + u] += (w * a[u]) * t;
   }
+}
+
+// H q = r for the n x n band of half-bandwidth 3 in Hb: banded Cholesky H = L L^T in place (L(i, k) in Hb[i][i - k]),
+// then the two triangular solves, q in r.  False on a pivot that is not finite and positive or a non-finite solution.
+__device__ __forceinline__ bool band_solve(double (*Hb)[4], double* r, int n) {
+  for (int j = 0; j < n; ++j) {
+    double dj = Hb[j][0];
+    for (int k = j < 3 ? 0 : j - 3; k < j; ++k) dj -= Hb[j][j - k] * Hb[j][j - k];
+    if (!(dj > 0.0 && dj <= 1.7976931348623157e308)) return false;
+    const double ljj = sqrt(dj);
+    Hb[j][0] = ljj;
+    for (int i = j + 1; i <= j + 3 && i < n; ++i) {
+      double s = Hb[i][i - j];
+      for (int k = i - 3; k < j; ++k)
+        if (k >= 0) s -= Hb[i][i - k] * Hb[j][j - k];
+      Hb[i][i - j] = s / ljj;
+    }
+  }
+  for (int j = 0; j < n; ++j) {  // L z = r
+    double s = r[j];
+    for (int k = j < 3 ? 0 : j - 3; k < j; ++k) s -= Hb[j][j - k] * r[k];
+    r[j] = s / Hb[j][0];
+  }
+  for (int j = n - 1; j >= 0; --j) {  // L^T q = z
+    double s = r[j];
+    for (int i = j + 1; i <= j + 3 && i < n; ++i) s -= Hb[i][i - j] * r[i];
+    r[j] = s / Hb[j][0];
+  }
+  bool fin = true;
+  for (int j = 0; j < n; ++j) fin = fin && isfinite(r[j]);
+  return fin;
 }
 
 // One warp per trajectory.  Lanes 0..10 evaluate the look-ahead differences of waypoints 1..11 with the check kernels'
@@ -572,45 +603,14 @@ __global__ void __launch_bounds__(TC_WPB * 32) yaw_explore_kernel(int B, int n, 
     const double jerk[4] = {-1.0, 3.0, -3.0, 1.0}, pos[3] = {1.0, 4.0, 1.0}, vel[3] = {-1.0, 0.0, 1.0},
                  acc[3] = {1.0, -2.0, 1.0};
     const double ws = prm.ld_smooth / (pt_dist * pt_dist), dt2 = dt_yaw * dt_yaw;
-    for (int i = 0; i + 3 < YP; ++i) yaw_term<4>(y, i, jerk, ws, 0.0);
-    yaw_term<3>(y, 0, pos, prm.ld_start * 10.0 / 36.0, 6.0 * y0);
-    yaw_term<3>(y, 0, vel, prm.ld_start / (4.0 * dt2), 2.0 * dt_yaw * y1);
-    yaw_term<3>(y, 0, acc, prm.ld_start / (dt2 * dt2), dt2 * y2);
-    yaw_term<3>(y, YS, pos, prm.ld_end / 36.0, 6.0 * ye);
-    yaw_term<3>(y, YS, vel, prm.ld_end / (4.0 * dt2), 0.0);
-    for (int i = 0; i < nw; ++i) yaw_term<3>(y, i + 1, pos, prm.ld_waypt / 36.0, 6.0 * y.wp[i]);
-    // banded Cholesky H = L L^T, L(i, k) in Hb[i][i - k]
-    for (int j = 0; j < YP && status == 0; ++j) {
-      double dj = y.Hb[j][0];
-      for (int k = j < 3 ? 0 : j - 3; k < j; ++k) dj -= y.Hb[j][j - k] * y.Hb[j][j - k];
-      if (!(dj > 0.0 && dj <= 1.7976931348623157e308)) {
-        status = FUELGPU_YAW_NOT_SPD;
-        break;
-      }
-      const double ljj = sqrt(dj);
-      y.Hb[j][0] = ljj;
-      for (int i = j + 1; i <= j + 3 && i < YP; ++i) {
-        double s = y.Hb[i][i - j];
-        for (int k = i - 3; k < j; ++k)
-          if (k >= 0) s -= y.Hb[i][i - k] * y.Hb[j][j - k];
-        y.Hb[i][i - j] = s / ljj;
-      }
-    }
-    if (status == 0) {
-      for (int j = 0; j < YP; ++j) {  // L z = r
-        double s = y.r[j];
-        for (int k = j < 3 ? 0 : j - 3; k < j; ++k) s -= y.Hb[j][j - k] * y.r[k];
-        y.r[j] = s / y.Hb[j][0];
-      }
-      for (int j = YP - 1; j >= 0; --j) {  // L^T q = z
-        double s = y.r[j];
-        for (int i = j + 1; i <= j + 3 && i < YP; ++i) s -= y.Hb[i][i - j] * y.r[i];
-        y.r[j] = s / y.Hb[j][0];
-      }
-      bool fin = true;
-      for (int j = 0; j < YP; ++j) fin = fin && isfinite(y.r[j]);
-      if (!fin) status = FUELGPU_YAW_NOT_SPD;
-    }
+    for (int i = 0; i + 3 < YP; ++i) yaw_term<4>(y.Hb, y.r, i, jerk, ws, 0.0);
+    yaw_term<3>(y.Hb, y.r, 0, pos, prm.ld_start * 10.0 / 36.0, 6.0 * y0);
+    yaw_term<3>(y.Hb, y.r, 0, vel, prm.ld_start / (4.0 * dt2), 2.0 * dt_yaw * y1);
+    yaw_term<3>(y.Hb, y.r, 0, acc, prm.ld_start / (dt2 * dt2), dt2 * y2);
+    yaw_term<3>(y.Hb, y.r, YS, pos, prm.ld_end / 36.0, 6.0 * ye);
+    yaw_term<3>(y.Hb, y.r, YS, vel, prm.ld_end / (4.0 * dt2), 0.0);
+    for (int i = 0; i < nw; ++i) yaw_term<3>(y.Hb, y.r, i + 1, pos, prm.ld_waypt / 36.0, 6.0 * y.wp[i]);
+    if (!band_solve(y.Hb, y.r, YP)) status = FUELGPU_YAW_NOT_SPD;
   }
 
   // what the reference defined before a failure is written, the rest is NaN
@@ -626,6 +626,153 @@ __global__ void __launch_bounds__(TC_WPB * 32) yaw_explore_kernel(int B, int n, 
   o.pt_dist = have_wp ? pt_dist : nan;
   o.n_waypt = have_wp ? nw : 0;
   o.status = status;
+  info[b] = o;
+}
+
+// ---- planYaw (planner_manager.cpp:695-772) on each trajectory of the batch ---------------------------------------------
+constexpr int PYS = FUELGPU_PLANYAW_MAX_SEG, PYP = FUELGPU_PLANYAW_MAX_PTS;
+constexpr int PY_WPB = 2;  // warps per CTA: 2 x sizeof(PlanYawSmem) stays under the 48 KB of static shared memory
+
+struct PlanYawSmem {
+  SplineSmem s;
+  double wp[PYS];     // atan2 of look-ahead difference i (NaN where |pd| <= 1e-6), then waypoint i
+  double Hb[PYP][4];  // normal equations, Hb[i][d] = H(i, i - d); the Cholesky factor in place
+  double r[PYP];      // right-hand side, then the solution
+};
+
+// One warp per trajectory.  Lanes l and l + 16 evaluate pc and pf of waypoints l, l + 16, ... with the check kernels'
+// deboor, lane 0 the velocity spline at duration - 0.1; lane 0 then chains calcNextYaw in the reference's order, builds
+// the initial guess and pt_dist_, assembles the normal equations of SMOOTHNESS | START | END (3 states) | WAYPOINTS
+// (dim_ == 1; the integer-coefficient form of yaw_explore_kernel) and solves them with band_solve.
+__global__ void __launch_bounds__(PY_WPB * 32) plan_yaw_kernel(int B, int n, int nvar, const double* __restrict__ x,
+                                                               const double* __restrict__ dtv,
+                                                               const double* __restrict__ syaw, FuelOptParams prm,
+                                                               double* __restrict__ yaw,
+                                                               FuelPlanYawInfo* __restrict__ info,
+                                                               double* __restrict__ wpt) {
+  __shared__ PlanYawSmem sm[PY_WPB];
+  const int lane = threadIdx.x & 31;
+  const int b = blockIdx.x * PY_WPB + (threadIdx.x >> 5);
+  if (b >= B) return;
+  PlanYawSmem& y = sm[threadIdx.x >> 5];
+  const double nan = __longlong_as_double(0x7ff8000000000000ll);
+
+  const double dt = nvar == 3 * n + 1 ? x[(size_t)b * nvar + 3 * n] : dtv[b];
+  const double y0 = syaw[3 * b], y1 = syaw[3 * b + 1], y2 = syaw[3 * b + 2];
+  int status = 0, seg = 0;
+  double duration = nan, dt_yaw = nan;
+  if (!(dt > 0.0 && dt <= 1.7976931348623157e308) || !isfinite(y1) || !isfinite(y2) ||
+      !(fabs(y0) <= FUELGPU_YAW_MAX_START)) {
+    status = FUELGPU_YAW_BAD_INPUT;
+  } else {
+    load_spline(y.s, b, n, nvar, x, dtv, lane);
+    duration = y.s.U[n] - y.s.U[3];  // getTimeSum
+    const double q = duration / 0.3;
+    if (!(duration > 0.0 && duration <= 1.7976931348623157e308)) status = FUELGPU_YAW_BAD_INPUT;
+    else if (!(q <= (double)PYS)) status = FUELGPU_YAW_TOO_LONG;
+    else {
+      seg = (int)ceil(q);
+      dt_yaw = duration / seg;
+    }
+  }
+  // waypoint i = base + l: lane l evaluates pc at tc, lane l + 16 pf at min(duration, tc + forward_t)
+  const int l = lane & 15;
+  for (int base = 0; base < seg; base += 16) {
+    const int i = base + l;
+    double p[3] = {0.0, 0.0, 0.0};
+    if (i < seg) {
+      const double tc = i * dt_yaw;
+      const double tf2 = tc + 2.0;
+      const double t = lane < 16 ? tc : tf2 < duration ? tf2 : duration;
+      int k = 3;
+      deboor<3>(y.s.P, y.s.U, n, t + y.s.U[3], &k, p);
+    }
+    const double dx = __shfl_down_sync(FULL, p[0], 16) - p[0], dy = __shfl_down_sync(FULL, p[1], 16) - p[1],
+                 dz = __shfl_down_sync(FULL, p[2], 16) - p[2];
+    if (lane < 16 && i < seg) y.wp[i] = sqrt((dx * dx + dy * dy) + dz * dz) > 1e-6 ? atan2(dy, dx) : nan;
+  }
+  __syncwarp();
+  if (lane != 0) return;
+
+  // the calcNextYaw chain from the unwrapped start yaw (:707-730)
+  double last_yaw = y0;
+  for (int i = 0; i < seg; ++i) {
+    double w = y.wp[i];
+    if (w != w) {  // waypt = waypts.back()
+      if (i == 0) {
+        status = FUELGPU_YAW_NO_LOOKAHEAD;
+        break;
+      }
+      w = y.wp[i - 1];
+    } else {
+      w = next_yaw(last_yaw, w);
+    }
+    last_yaw = w;
+    y.wp[i] = w;
+  }
+  const int np = seg + 3;
+  double pt_dist = nan, ye = nan;
+  if (status == 0) {
+    // velocity_traj_.evaluateDeBoorT(duration - 0.1); evaluateDeBoor clamps it to the first knot when duration < 0.1.
+    // CUDA's atan2 has C99's signed-zero cases, so atan2(+-0, -0) = +-pi as in glibc.
+    double v[3];
+    int k = 2;
+    deboor<2>(y.s.Q, y.s.U + 1, n - 1, (duration - 0.1) + y.s.U[3], &k, v);
+    ye = next_yaw(last_yaw, atan2(v[1], v[0]));
+    // the initial guess: states2pts * start_yaw in rows 0-2, then states2pts * (end, 0, 0) in rows seg..seg+2
+    const double c13 = ((1 / 3.0) * dt_yaw) * dt_yaw, c16 = ((-(1 / 6.0)) * dt_yaw) * dt_yaw;
+    const double gs[3] = {(1.0 * y0 + -dt_yaw * y1) + c13 * y2, (1.0 * y0 + 0.0 * y1) + c16 * y2,
+                          (1.0 * y0 + dt_yaw * y1) + c13 * y2};
+    const double ge[3] = {(1.0 * ye + -dt_yaw * 0.0) + c13 * 0.0, (1.0 * ye + 0.0 * 0.0) + c16 * 0.0,
+                          (1.0 * ye + dt_yaw * 0.0) + c13 * 0.0};
+    auto pick = [](const double (&v)[3], int k) { return k == 0 ? v[0] : k == 1 ? v[1] : v[2]; };  // no local memory
+    auto g = [&](int i) { return i >= seg ? pick(ge, i - seg) : i < 3 ? pick(gs, i) : 0.0; };
+    double d = 0.0;  // pt_dist_ (bspline_optimizer.cpp:136-140) over the seg + 3 rows
+    for (int i = 0; i + 1 < np; ++i) {
+      const double e = g(i + 1) - g(i);
+      d += sqrt(e * e);
+    }
+    pt_dist = d / (double)np;
+    if (pt_dist == 0.0) status = FUELGPU_YAW_ZERO_PT_DIST;
+  }
+
+  if (status == 0) {
+    for (int i = 0; i < np; ++i) {
+      y.r[i] = 0.0;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) y.Hb[i][k] = 0.0;
+    }
+    const double jerk[4] = {-1.0, 3.0, -3.0, 1.0}, pos[3] = {1.0, 4.0, 1.0}, vel[3] = {-1.0, 0.0, 1.0},
+                 acc[3] = {1.0, -2.0, 1.0};
+    const double ws = prm.ld_smooth / (pt_dist * pt_dist), dt2 = dt_yaw * dt_yaw;
+    for (int i = 0; i + 3 < np; ++i) yaw_term<4>(y.Hb, y.r, i, jerk, ws, 0.0);
+    yaw_term<3>(y.Hb, y.r, 0, pos, prm.ld_start * 10.0 / 36.0, 6.0 * y0);
+    yaw_term<3>(y.Hb, y.r, 0, vel, prm.ld_start / (4.0 * dt2), 2.0 * dt_yaw * y1);
+    yaw_term<3>(y.Hb, y.r, 0, acc, prm.ld_start / (dt2 * dt2), dt2 * y2);
+    yaw_term<3>(y.Hb, y.r, seg, pos, prm.ld_end / 36.0, 6.0 * ye);
+    yaw_term<3>(y.Hb, y.r, seg, vel, prm.ld_end / (4.0 * dt2), 0.0);
+    yaw_term<3>(y.Hb, y.r, seg, acc, prm.ld_end / (dt2 * dt2), 0.0);
+    for (int i = 0; i < seg; ++i) yaw_term<3>(y.Hb, y.r, i, pos, prm.ld_waypt / 36.0, 6.0 * y.wp[i]);
+    if (!band_solve(y.Hb, y.r, np)) status = FUELGPU_YAW_NOT_SPD;
+  }
+
+  // what the reference defined before a failure is written, the rest is NaN
+  const bool have_seg = status == 0 || status == FUELGPU_YAW_NO_LOOKAHEAD || status == FUELGPU_YAW_ZERO_PT_DIST ||
+                        status == FUELGPU_YAW_NOT_SPD;
+  const bool have_wp = status == 0 || status == FUELGPU_YAW_ZERO_PT_DIST || status == FUELGPU_YAW_NOT_SPD;
+  double* yb = yaw + (size_t)b * PYP;
+  for (int j = 0; j < PYP; ++j) yb[j] = status == 0 && j < np ? y.r[j] : nan;
+  if (wpt) {
+    double* wb = wpt + (size_t)b * PYS;
+    for (int i = 0; i < PYS; ++i) wb[i] = !have_wp ? nan : i < seg ? y.wp[i] : 0.0;
+  }
+  FuelPlanYawInfo o;
+  o.dt_yaw = have_seg ? dt_yaw : nan;
+  o.pt_dist = have_wp ? pt_dist : nan;
+  o.seg_num = have_seg ? seg : 0;
+  o.n_waypt = have_wp ? seg : 0;
+  o.status = status;
+  o.reserved = 0;
   info[b] = o;
 }
 
@@ -673,6 +820,18 @@ int yaw_explore_impl(FuelMap* m, int B, int n_pts, int nvar, const double* x_dev
   const int grid = (B + TC_WPB - 1) / TC_WPB;
   yaw_explore_kernel<<<grid, TC_WPB * 32, 0, m->stream>>>(B, n_pts, nvar, x_dev, dt_dev, syaw_dev, eyaw_dev, *p, *yp,
                                                           yaw_dev, info_dev, wpt_dev);
+  FUEL_CUDA(m, cudaGetLastError());
+  FUEL_LAUNCHES(m, 1);
+  return 0;
+}
+
+int plan_yaw_impl(FuelMap* m, int B, int n_pts, int nvar, const double* x_dev, const double* dt_dev,
+                  const double* syaw_dev, const FuelOptParams* p, double* yaw_dev, FuelPlanYawInfo* info_dev,
+                  double* wpt_dev) {
+  if (B == 0) return 0;
+  const int grid = (B + PY_WPB - 1) / PY_WPB;
+  plan_yaw_kernel<<<grid, PY_WPB * 32, 0, m->stream>>>(B, n_pts, nvar, x_dev, dt_dev, syaw_dev, *p, yaw_dev, info_dev,
+                                                       wpt_dev);
   FUEL_CUDA(m, cudaGetLastError());
   FUEL_LAUNCHES(m, 1);
   return 0;

@@ -4,7 +4,8 @@ fuelgpu_kino_search_batch.
 
 kino_search_batch runs B replans' searches -- the close-goal refusal, search(init = true), the retry at init = false and
 getSamples -- and returns the arrays fuelgpu_bspline_parameterize_batch takes.  kinodynamic_replan_batch carries them
-on through parameterizeToBspline, getBoundaryStates and the solver, like plan_explore_traj_batch.  KinodynamicAstar is
+on through parameterizeToBspline and getBoundaryStates, and kino_replan_traj_batch through the solver and planYaw, like
+plan_explore_traj_batch.  KinodynamicAstar is
 the reference's class over one search; only the non-dynamic search exists (FUEL's exploration never asks for another).
 """
 import ctypes as C
@@ -86,6 +87,36 @@ def kinodynamic_replan_batch(sdf_map, start, vel, acc, goal, time_lb=None, **par
         x, traj = parameterize_batch(sdf_map, res["points"][rows, :K], res["derivs"][rows], res["dt"][rows], tlb)
         groups.append((rows, x, traj))
     return res, groups
+
+
+def kino_replan_traj_batch(sdf_map, start, vel, acc, goal, opt, solve, start_yaw, time_lb=None, **params):
+    """KinoReplanFSM::callKinodynamicReplan's planner calls for B replans: kinodynamicReplan(start, vel, acc, goal, 0,
+    time_lb) -- kinodynamic_replan_batch, then opt.optimizeBatch on each point count's group -- and planYaw(start_yaw)
+    (polynomial_traj.plan_yaw_batch) on each group's solver output.
+    opt: a BsplineOptimizer set up on `sdf_map`; solve: keyword arguments of optimizeBatch besides x / traj_consts /
+    n_pts, with cost_function (NORMAL_PHASE, with MINTIME where manager/min_time sets it); start_yaw: [3] or [B, 3].
+    Returns dict(res: the kino_search_batch dict, x: a list of [nvar] solver outputs or None per row, yaw [B, 131],
+    yaw_info [B] of PLANYAW_INFO_DTYPE); rows without samples keep None, NaN yaw and status -1."""
+    from .polynomial_traj import PLANYAW_INFO_DTYPE, PLANYAW_MAX_PTS, plan_yaw_batch
+    res, groups = kinodynamic_replan_batch(sdf_map, start, vel, acc, goal, time_lb, **params)
+    B = len(res["info"])
+    sy = np.broadcast_to(np.asarray(start_yaw, dtype=np.float64), (B, 3))
+    mask = int(solve["cost_function"])
+    mintime = bool(mask & opt.MINTIME)
+    kw = {k: v for k, v in solve.items() if k != "cost_function"}
+    xs = [None] * B
+    yaw = np.full((B, PLANYAW_MAX_PTS), np.nan)
+    yaw_info = np.zeros(B, dtype=PLANYAW_INFO_DTYPE)
+    yaw_info["dt_yaw"] = yaw_info["pt_dist"] = np.nan
+    yaw_info["status"] = -1
+    for rows, x0, tc in groups:
+        n = (x0.shape[1] - 1) // 3
+        dt = None if mintime else x0[:, 3 * n].copy()
+        x, _, _ = opt.optimizeBatch(x0 if mintime else np.ascontiguousarray(x0[:, :3 * n]), tc, n, mask, **kw)
+        yaw[rows], yaw_info[rows], _ = plan_yaw_batch(sdf_map, x, n, sy[rows], opt, dt=dt)
+        for r, b in enumerate(rows):
+            xs[b] = x[r].copy()
+    return dict(res=res, x=xs, yaw=yaw, yaw_info=yaw_info)
 
 
 class KinodynamicAstar:

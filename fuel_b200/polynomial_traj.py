@@ -6,6 +6,8 @@ waypoints_batch runs the polynomial stage: segment times, waypointsTraj, getTota
 samples and boundary derivatives parameterizeToBspline takes.  plan_explore_traj_batch chains it with
 parameterize_batch -> BsplineOptimizer.optimizeBatch -> check_batch, one launch per point count.
 plan_yaw_explore_batch is planYawExplore (:774-865) on every trajectory of a solver batch (fuelgpu_yaw_explore_batch).
+plan_yaw_batch is planYaw (:695-772), the kinodynamic replan's yaw, on every trajectory of a solver batch
+(fuelgpu_plan_yaw_batch).
 """
 import ctypes as C
 
@@ -22,6 +24,10 @@ YAW_SEG_NUM, YAW_PTS, YAW_MAX_WAYPT = 12, 15, 11  # FUELGPU_YAW_SEG_NUM, _PTS, _
 YAW_OK, YAW_BAD_INPUT, YAW_RELAX_OVERFLOW, YAW_NO_LOOKAHEAD, YAW_ZERO_PT_DIST, YAW_NOT_SPD = 0, 1, 2, 3, 4, 5
 YAW_INFO_DTYPE = np.dtype([("dt_yaw", np.float64), ("pt_dist", np.float64), ("n_waypt", np.int32),
                            ("status", np.int32)])
+PLANYAW_MAX_SEG, PLANYAW_MAX_PTS = 128, 131  # FUELGPU_PLANYAW_MAX_SEG, _MAX_PTS
+YAW_TOO_LONG = 6  # FUELGPU_YAW_TOO_LONG (plan_yaw_batch only)
+PLANYAW_INFO_DTYPE = np.dtype([("dt_yaw", np.float64), ("pt_dist", np.float64), ("seg_num", np.int32),
+                               ("n_waypt", np.int32), ("status", np.int32), ("reserved", np.int32)])
 
 # one FuelPolyInfo per tour (include/fuelgpu.h)
 INFO_DTYPE = np.dtype([("duration", np.float64), ("length", np.float64), ("dt", np.float64), ("seg_num", np.int32),
@@ -147,6 +153,28 @@ def plan_yaw_explore_batch(sdf_map, x, n_pts, start_yaw, end_yaw, opt_params, re
     h = _handle(sdf_map)
     check(lib().fuelgpu_yaw_explore_batch(h, B, n_pts, x.shape[1], ptr(x), ptr(dt), ptr(sy), ptr(ey), C.byref(prm),
                                           C.byref(yp), ptr(yaw), ptr(info), ptr(waypt)), h)
+    return yaw, info, waypt
+
+
+def plan_yaw_batch(sdf_map, x, n_pts, start_yaw, opt_params, dt=None):
+    """planYaw(start_yaw) (planner_manager.cpp:695-772) with every trajectory of a batch as the position trajectory, on
+    the device of `sdf_map` (fuelgpu_plan_yaw_batch).
+    x: [B, nvar] in the solver's layout (dt in the last column, or dt [B] given); start_yaw: [3] or [B, 3] (yaw, yawdot,
+    yawddot; the yaw is used as given); opt_params: a FuelOptParams or a BsplineOptimizer (ld_smooth, ld_start, ld_end and
+    ld_waypt are read).
+    Returns (yaw [B, 131]: the seg_num + 3 control points of the yaw spline with knot span info['dt_yaw'], NaN after them,
+    info [B] of PLANYAW_INFO_DTYPE, waypt [B, 128]: plan_data_.path_yaw_, zero past info['n_waypt']).  A trajectory with
+    info['status'] != 0 has NaN yaw (include/fuelgpu.h lists the statuses)."""
+    x, dt = _inputs(x, n_pts, dt)
+    B = x.shape[0]
+    sy = np.ascontiguousarray(np.broadcast_to(np.asarray(start_yaw, dtype=np.float64), (B, 3)))
+    prm = opt_params if isinstance(opt_params, FuelOptParams) else opt_params.params_
+    yaw = np.empty((B, PLANYAW_MAX_PTS))
+    info = np.empty(B, dtype=PLANYAW_INFO_DTYPE)
+    waypt = np.empty((B, PLANYAW_MAX_SEG))
+    h = _handle(sdf_map)
+    check(lib().fuelgpu_plan_yaw_batch(h, B, n_pts, x.shape[1], ptr(x), ptr(dt), ptr(sy), C.byref(prm), ptr(yaw),
+                                       ptr(info), ptr(waypt)), h)
     return yaw, info, waypt
 
 

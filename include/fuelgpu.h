@@ -577,6 +577,64 @@ FUELGPU_API int fuelgpu_yaw_explore_batch_dev(FuelMap* map, int32_t B, int32_t n
                                               const FuelOptParams* params, const FuelYawParams* yaw_params,
                                               void* yaw_dev, void* info_dev, void* waypt_dev);
 
+/* ---- kinodynamic-replan yaw: planYaw on the device ---------------------------------------------------------------------
+ * Replaces FastPlannerManager::planYaw(start_yaw) (plan_manage/src/planner_manager.cpp:695-772, calcNextYaw :867-885),
+ * the last stage of KinoReplanFSM::callKinodynamicReplan (kino_replan_fsm.cpp:280-300), for every trajectory of a batch
+ * in the solver's layout (as fuelgpu_yaw_explore_batch: x [B][nvar], n_pts 4..FUELGPU_MAX_PTS, dt in the last column
+ * when nvar == 3*n_pts + 1, else dt [B]).  Per trajectory, with duration = getTimeSum():
+ *   seg_num = ceil(duration / 0.3), dt_yaw = duration / seg_num;
+ *   waypoint i = 0 .. seg_num - 1: atan2 of evaluateDeBoorT(min(duration, tc + 2)) - evaluateDeBoorT(tc) at
+ *   tc = i * dt_yaw, chained through calcNextYaw from start_yaw[0] as given (not wrapped), or the previous waypoint
+ *   where |pd| <= 1e-6; waypoint i constrains control points i..i+2;
+ *   end yaw: atan2 of the velocity spline (getDerivative(), updateTrajInfo :518-526) at evaluateDeBoorT(duration - 0.1),
+ *   clamped to the spline's first knot as evaluateDeBoor does when duration < 0.1, then calcNextYaw;
+ *   the (seg_num + 3) x 1 initial guess: states2pts * start_yaw in rows 0-2, states2pts * (end, 0, 0) in rows
+ *   seg_num..seg_num+2, written second (for seg_num 1 and 2 the blocks overlap and the end block wins); pt_dist_ of it;
+ *   the minimizer of SMOOTHNESS | START | END | WAYPOINTS with three end states (end velocity and acceleration 0, so
+ *   calcEndCost's acceleration term is active, bspline_optimizer.cpp:393-431), combineCost with dim_ == 1.
+ * Divergences from the reference, as for planYawExplore (DESIGN.md 4.15): the strictly convex quadratic objective is
+ * solved by a banded Cholesky factorization in fp64 instead of NLopt (NLopt parity unpinned); |pd| is summed
+ * (dx*dx + dy*dy) + dz*dz and states2pts * v left to right per row; the device's atan2 is within 2 ulp of the C
+ * library's, so the waypoints agree to that rounding, and given them the end yaw, the initial guess and pt_dist are bit
+ * for bit.  seg_num, dt_yaw and the waypoint count equal the reference's fp64 arithmetic bit for bit.
+ *   start_yaw [B][3]   yaw, yawdot, yawddot (finite, |yaw| <= FUELGPU_YAW_MAX_START)
+ *   params             ld_smooth, ld_start, ld_end and ld_waypt are read (ld_smooth and ld_start finite and > 0)
+ * Outputs: yaw [B][FUELGPU_PLANYAW_MAX_PTS] (control points of the yaw spline, knot span info[b].dt_yaw; NaN past
+ * seg_num + 3); info [B]; waypt [B][FUELGPU_PLANYAW_MAX_SEG] or NULL (plan_data_.path_yaw_, zero past n_waypt).
+ * Where the reference's behaviour is undefined, or the trajectory is longer than this library's cap, a trajectory gets a
+ * status and NaN yaw.  What the reference computed before that point is written (seg_num and dt_yaw from
+ * FUELGPU_YAW_NO_LOOKAHEAD on; pt_dist, n_waypt and the waypoints for FUELGPU_YAW_ZERO_PT_DIST and FUELGPU_YAW_NOT_SPD),
+ * the rest is NaN, seg_num and n_waypt 0:
+ *   FUELGPU_YAW_BAD_INPUT       (_dev only) a dt or start yaw the host entry refuses; also (either entry) a duration that
+ *                               is not finite and positive (the reference's seg_num is 0 and dt_yaw 0/0)
+ *   FUELGPU_YAW_TOO_LONG        duration / 0.3 > FUELGPU_PLANYAW_MAX_SEG (tested before the int conversion)
+ *   FUELGPU_YAW_NO_LOOKAHEAD    |pd| <= 1e-6 at i = 0 (a hovering start): the reference reads waypts.back() of an empty
+ *                               vector
+ *   FUELGPU_YAW_ZERO_PT_DIST    pt_dist_ == 0 (start yaw, rate and acceleration 0 and an end velocity along +x): every
+ *                               cost of the reference is NaN
+ *   FUELGPU_YAW_NOT_SPD         a pivot that is not finite and positive in the factorization
+ * Runs on the map's main stream, so fuelgpu_bspline_optimize_batch_dev -> fuelgpu_plan_yaw_batch_dev needs no host sync.
+ * The host entry returns FUELGPU_EINVAL and writes nothing on B < 0, a bad n_pts or nvar, a dt that is not finite and
+ * positive, a start yaw that is not finite or has |yaw| > FUELGPU_YAW_MAX_START, or a bad parameter; the _dev entry
+ * checks the parameters alone and marks a bad trajectory FUELGPU_YAW_BAD_INPUT, leaving the others unaffected.  Not timed
+ * in fuelgpu_map_last_timing. */
+#define FUELGPU_PLANYAW_MAX_SEG 128 /* 38.4 s of trajectory at 0.3 s per segment */
+#define FUELGPU_PLANYAW_MAX_PTS (FUELGPU_PLANYAW_MAX_SEG + 3)
+#define FUELGPU_YAW_TOO_LONG 6
+typedef struct {
+  double dt_yaw, pt_dist; /* knot span of the yaw spline; pt_dist_ of the initial guess */
+  int32_t seg_num;        /* 1..FUELGPU_PLANYAW_MAX_SEG; the yaw spline has seg_num + 3 control points */
+  int32_t n_waypt;        /* waypoints (= seg_num when planned) */
+  int32_t status;         /* 0 or FUELGPU_YAW_* */
+  int32_t reserved;
+} FuelPlanYawInfo;
+FUELGPU_API int fuelgpu_plan_yaw_batch(FuelMap* map, int32_t B, int32_t n_pts, int32_t nvar, const double* x,
+                                       const double* dt, const double* start_yaw, const FuelOptParams* params,
+                                       double* yaw, FuelPlanYawInfo* info, double* waypt);
+FUELGPU_API int fuelgpu_plan_yaw_batch_dev(FuelMap* map, int32_t B, int32_t n_pts, int32_t nvar, const void* x_dev,
+                                           const void* dt_dev, const void* start_yaw_dev, const FuelOptParams* params,
+                                           void* yaw_dev, void* info_dev, void* waypt_dev);
+
 /* ---- geometric path to the next viewpoint: Astar::search, shortenPath and the goal branch on the device -------------
  * Replaces, for B (start, goal) queries, the head of FastExplorationManager::planExploreMotion
  * (exploration_manager/src/fast_exploration_manager.cpp:238-263): path_finder_->reset(), Astar::search(pos, next_pos)
